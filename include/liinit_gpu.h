@@ -103,11 +103,20 @@ int liinit_raw_upload(liinit_ctx* h, const float* pts, int stride_floats, int ti
  * omega = state.bias_g (angular velocity), rot_end / vel_end = the PROPAGATED state. In place on the staged cloud. */
 int liinit_raw_undistort_cv(liinit_ctx* h, const double omega[3], const double rot_end[9], const double vel_end[3]);
 /* propagation_and_undist's back-propagation loop (IMU_Processing.hpp:390-415). poses: the IMUpose table, npose x 22 doubles
- * {offset_time, acc[3], gyr[3], vel[3], pos[3], rot[9]} (Pose6D, common_lib.h:184-199); the state is the propagated one. */
+ * {offset_time, acc[3], gyr[3], vel[3], pos[3], rot[9]} (Pose6D, common_lib.h:184-199); the state is the propagated one.
+ * 2 <= npose <= LIINIT_MAX_IMU_POSES. */
+#define LIINIT_MAX_IMU_POSES 4096
 int liinit_raw_undistort_imu(liinit_ctx* h, const double* poses, int npose, const double rot_end[9], const double pos_end[3],
                              const double R_LI[9], const double T_LI[3]);
 /* The staged raw cloud as packed xyz (after whatever undistortion ran). */
 int liinit_raw_download(liinit_ctx* h, float* xyz, int cap_points, int* n);
+/* The staged (undistorted) raw cloud in the world frame, packed xyz in upload order: pointBodyToWorld (laserMapping.cpp:209-220)
+ * with the given state, the same arithmetic as the map update. This is feats_undistort as publish_frame_world publishes it with
+ * dense_publish_en (:563) and as pcd_save accumulates it (:594-603); intensities can be joined by index on the host.
+ * *n = number of staged points; xyz may be NULL to ask for it. LIINIT_ERR_CAPACITY when cap_points < *n (nothing is written),
+ * LIINIT_ERR_INVALID when no raw cloud is staged. */
+int liinit_raw_download_world(liinit_ctx* h, const double rot_end[9], const double pos_end[3], const double R_LI[9], const double T_LI[3],
+                              float* xyz, int cap_points, int* n);
 /* downSizeFilterSurf.filter (laserMapping.cpp:917-918): voxel grid over the staged cloud -> the resident scan. */
 int liinit_raw_downsample(liinit_ctx* h, float leaf_size, int* n_down);
 /* Raw (undistorted, not yet downsampled) scan: voxel-grid filter on the device, then the result becomes the resident scan.

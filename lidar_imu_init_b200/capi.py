@@ -34,7 +34,7 @@ _i32 = np.ctypeslib.ndpointer(dtype=np.int32, flags="C_CONTIGUOUS")
 SYMBOLS = [
     "liinit_create", "liinit_destroy", "liinit_last_error", "liinit_set_stream", "liinit_map_build", "liinit_map_add_points", "liinit_map_delete_boxes",
     "liinit_map_compact", "liinit_map_validnum", "liinit_map_size", "liinit_map_download", "liinit_map_nearest_search", "liinit_scan_upload", "liinit_scan_attach_host", "liinit_scan_upload_raw", "liinit_scan_download_body", "liinit_raw_upload", "liinit_raw_undistort_cv", "liinit_raw_undistort_imu",
-    "liinit_raw_download", "liinit_raw_downsample",
+    "liinit_raw_download", "liinit_raw_download_world", "liinit_raw_downsample",
     "liinit_icp_iterate", "liinit_icp_iterate_device", "liinit_scan_download_effect", "liinit_scan_download_state",
     "liinit_map_incremental", "liinit_last_pass_timing", "liinit_last_pass_kernel_times", "liinit_launch_count", "liinit_map_stats", "liinit_knn_index",
     "liinit_comm_unique_id", "liinit_comm_init", "liinit_comm_info", "liinit_comm_last_local", "liinit_comm_mode", "liinit_debug_esti_plane", "liinit_set_reseed",
@@ -77,6 +77,7 @@ def load():
     L.liinit_raw_undistort_cv.argtypes = [vp, _f64, _f64, _f64]
     L.liinit_raw_undistort_imu.argtypes = [vp, _f64, C.c_int, _f64, _f64, _f64, _f64]
     L.liinit_raw_download.argtypes = [vp, vp, C.c_int, C.POINTER(C.c_int)]
+    L.liinit_raw_download_world.argtypes = [vp, _f64, _f64, _f64, _f64, vp, C.c_int, C.POINTER(C.c_int)]
     L.liinit_raw_downsample.argtypes = [vp, C.c_float, C.POINTER(C.c_int)]
     L.liinit_scan_download_body.argtypes = [vp, vp, C.c_int, C.POINTER(C.c_int)]
     L.liinit_icp_iterate.argtypes = [vp, _f64, _f64, _f64, _f64, C.c_int, C.c_int, _f64, _f64, C.POINTER(C.c_int), C.POINTER(C.c_double)]
@@ -236,6 +237,16 @@ class LiInitGpu:
         out = np.zeros((max(getattr(self, "raw_n", 0), 1), 3), np.float32)
         self._ck(self.L.liinit_raw_download(self.h, _ptr(out), len(out), C.byref(n)))
         return out[:n.value]
+
+    def raw_world(self, rot_end, pos_end, R_LI, T_LI):
+        """The staged (undistorted) raw cloud in the world frame, [n, 3] float32 in upload order (pointBodyToWorld)."""
+        n = C.c_int(0)
+        args = (np.ascontiguousarray(rot_end, np.float64).reshape(9), np.ascontiguousarray(pos_end, np.float64),
+                np.ascontiguousarray(R_LI, np.float64).reshape(9), np.ascontiguousarray(T_LI, np.float64))
+        self._ck(self.L.liinit_raw_download_world(self.h, *args, None, 0, C.byref(n)))
+        out = np.zeros((n.value, 3), np.float32)
+        self._ck(self.L.liinit_raw_download_world(self.h, *args, _ptr(out), n.value, C.byref(n)))
+        return out
 
     def raw_downsample(self, leaf_size: float) -> int:
         nd = C.c_int(0)

@@ -266,6 +266,159 @@ void liinit_propagate_cv(liinit_state* s, double dt, const double* cov_gyr_scale
     for (int i = 0; i < 3; i++) s->pos_end[i] += s->vel_end[i] * dt;
 }
 
+void liinit_imu_init(liinit_imu* imu) {
+    std::memset(imu, 0, sizeof(*imu));
+    for (int i = 0; i < 3; i++) {
+        imu->cov_acc[i] = imu->cov_gyr[i] = 0.1;                 // IMU_Processing.hpp:97-102
+        imu->cov_R_LI[i] = 0.00001;
+        imu->cov_T_LI[i] = 0.0001;
+        imu->cov_bias_gyr[i] = imu->cov_bias_acc[i] = 0.0001;
+        imu->cov_acc_scale[i] = imu->cov_gyr_scale[i] = 0.1;     // the node's gyr_cov / acc_cov defaults (laserMapping.cpp:76)
+    }
+    imu->mean_acc_norm = 9.81;                                   // the node's mean_acc_norm default (:94)
+    imu->need_init = 1;
+}
+
+void liinit_imu_set_gyr_cov(liinit_imu* imu, const double* v) { std::memcpy(imu->cov_gyr_scale, v, 3 * sizeof(double)); }
+void liinit_imu_set_acc_cov(liinit_imu* imu, const double* v) { std::memcpy(imu->cov_acc_scale, v, 3 * sizeof(double)); }
+void liinit_imu_set_R_LI_cov(liinit_imu* imu, const double* v) { std::memcpy(imu->cov_R_LI, v, 3 * sizeof(double)); }
+void liinit_imu_set_T_LI_cov(liinit_imu* imu, const double* v) { std::memcpy(imu->cov_T_LI, v, 3 * sizeof(double)); }
+void liinit_imu_set_gyr_bias_cov(liinit_imu* imu, const double* v) { std::memcpy(imu->cov_bias_gyr, v, 3 * sizeof(double)); }
+void liinit_imu_set_acc_bias_cov(liinit_imu* imu, const double* v) { std::memcpy(imu->cov_bias_acc, v, 3 * sizeof(double)); }
+void liinit_imu_set_mean_acc_norm(liinit_imu* imu, double m) { imu->mean_acc_norm = m; }
+
+int liinit_imu_switch(liinit_imu* imu, const double* smp, int n) {
+    if (!imu || n < 0 || (n > 0 && !smp)) return LIINIT_ERR_INVALID;
+    if (n == 0) return LIINIT_OK;
+    std::memcpy(imu->last_imu, smp + (size_t)(n - 1) * LIINIT_IMU_SAMPLE_DOUBLES, sizeof(imu->last_imu));   // :448-451
+    imu->need_init = 0;
+    std::memcpy(imu->cov_acc, imu->cov_acc_scale, sizeof(imu->cov_acc));
+    std::memcpy(imu->cov_gyr, imu->cov_gyr_scale, sizeof(imu->cov_gyr));
+    return LIINIT_OK;
+}
+
+static void put_pose6d(double* o, double t, const double* a, const double* g, const double* v, const double* p, const double* R) {
+    o[0] = t;   // set_pose6d (common_lib.h:184-199)
+    for (int i = 0; i < 3; i++) {
+        o[1 + i] = a[i];
+        o[4 + i] = g[i];
+        o[7 + i] = v[i];
+        o[10 + i] = p[i];
+    }
+    std::memcpy(o + 13, R, 9 * sizeof(double));
+}
+
+int liinit_imu_propagate(liinit_imu* imu, liinit_state* s, const double* smp, int n, double pcl_beg_time, double pcl_end_offset_ms,
+                         double* poses, int* npose) {
+    if (!imu || !s || !npose || n < 0 || (n > 0 && (!smp || !poses))) return LIINIT_ERR_INVALID;
+    *npose = 0;
+    if (n == 0) return LIINIT_OK;
+    if (imu->need_init) return LIINIT_ERR_INVALID;
+    const double G_m_s2 = 9.81;   // common_lib.h:23
+    const double last_end = imu->last_lidar_end_time;
+    // v_imu = {last_imu_, samples...} (IMU_Processing.hpp:273-274); pair k = (v_imu[k], v_imu[k + 1])
+    auto sample = [&](int k) { return k == 0 ? imu->last_imu : smp + (size_t)(k - 1) * LIINIT_IMU_SAMPLE_DOUBLES; };
+    int np = 1;
+    for (int k = 0; k < n; k++) np += !(sample(k + 1)[0] < last_end);
+    if (np > LIINIT_MAX_IMU_POSES) return LIINIT_ERR_CAPACITY;
+    const double imu_end_time = sample(n)[0];
+    const double pcl_end_time = pcl_beg_time + pcl_end_offset_ms / double(1000);   // :288
+
+    put_pose6d(poses, 0.0, imu->acc_s_last, imu->angvel_last, s->vel_end, s->pos_end, s->rot_end);   // :293-294
+    double R[9], vel[3], pos[3], acc_imu[3] = {0, 0, 0}, angvel[3] = {0, 0, 0};   // (never read unset: the table would have one pose)
+    std::memcpy(R, s->rot_end, sizeof(R));
+    std::memcpy(vel, s->vel_end, sizeof(vel));
+    std::memcpy(pos, s->pos_end, sizeof(pos));
+    double* P = s->cov;
+    double T[D * D];
+    int out = 1;
+    for (int k = 0; k < n; k++) {
+        const double* head = sample(k);
+        const double* tail = sample(k + 1);
+        if (tail[0] < last_end) continue;   // :307
+        double acc[3];
+        for (int i = 0; i < 3; i++) {
+            angvel[i] = 0.5 * (head[1 + i] + tail[1 + i]);
+            acc[i] = 0.5 * (head[4 + i] + tail[4 + i]);
+            angvel[i] -= s->bias_g[i];                                   // :322
+            acc[i] = acc[i] / imu->mean_acc_norm * G_m_s2 - s->bias_a[i];   // :323
+        }
+        const double dt = (head[0] < last_end) ? tail[0] - last_end : tail[0] - head[0];   // :325-328
+        double Ef[9], Eb[9];
+        so3_exp_dt(angvel, dt, Ef);
+        so3_exp_dt(angvel, -dt, Eb);
+        // F (:335-343) is the identity except in rows 0:3 (Exp(-dt) at 0, -dt I at 15), 3:6 (dt I at 12) and 12:15
+        // (A = -R [acc]x dt at 0, -R dt at 18, dt I at 21). F P F^T is formed as T = F P, then T F^T; both sum in column order.
+        const double K[9] = {0, -acc[2], acc[1], acc[2], 0, -acc[0], -acc[1], acc[0], 0};
+        double nR[9], A[9], B[9];
+        for (int i = 0; i < 9; i++) nR[i] = -R[i];
+        mul33(nR, K, A);
+        for (int i = 0; i < 9; i++) {
+            A[i] *= dt;
+            B[i] = nR[i] * dt;
+        }
+        std::memcpy(T, P, sizeof(T));
+        for (int c = 0; c < D; c++)
+            for (int i = 0; i < 3; i++) {
+                T[i * D + c] = Eb[3 * i] * P[c] + Eb[3 * i + 1] * P[D + c] + Eb[3 * i + 2] * P[2 * D + c] + (-dt) * P[(15 + i) * D + c];
+                T[(3 + i) * D + c] = P[(3 + i) * D + c] + dt * P[(12 + i) * D + c];
+                T[(12 + i) * D + c] = A[3 * i] * P[c] + A[3 * i + 1] * P[D + c] + A[3 * i + 2] * P[2 * D + c] + P[(12 + i) * D + c] +
+                                      B[3 * i] * P[18 * D + c] + B[3 * i + 1] * P[19 * D + c] + B[3 * i + 2] * P[20 * D + c] +
+                                      dt * P[(21 + i) * D + c];
+            }
+        std::memcpy(P, T, sizeof(T));
+        for (int r = 0; r < D; r++) {
+            const double* t = T + r * D;
+            for (int i = 0; i < 3; i++) {
+                P[r * D + i] = t[0] * Eb[3 * i] + t[1] * Eb[3 * i + 1] + t[2] * Eb[3 * i + 2] + t[15 + i] * (-dt);
+                P[r * D + 3 + i] = t[3 + i] + t[12 + i] * dt;
+                P[r * D + 12 + i] = t[0] * A[3 * i] + t[1] * A[3 * i + 1] + t[2] * A[3 * i + 2] + t[12 + i] + t[18] * B[3 * i] +
+                                    t[19] * B[3 * i + 1] + t[20] * B[3 * i + 2] + t[21 + i] * dt;
+            }
+        }
+        // Q (:345-350); the acceleration block is R diag(cov_acc) R^T dt^2
+        for (int i = 0; i < 3; i++) {
+            P[i * D + i] += imu->cov_gyr[i] * dt * dt;
+            P[(6 + i) * D + 6 + i] += imu->cov_R_LI[i] * dt * dt;
+            P[(9 + i) * D + 9 + i] += imu->cov_T_LI[i] * dt * dt;
+            P[(15 + i) * D + 15 + i] += imu->cov_bias_gyr[i] * dt * dt;
+            P[(18 + i) * D + 18 + i] += imu->cov_bias_acc[i] * dt * dt;
+            for (int j = 0; j < 3; j++) {
+                double q = R[3 * i] * imu->cov_acc[0] * R[3 * j] + R[3 * i + 1] * imu->cov_acc[1] * R[3 * j + 1] +
+                           R[3 * i + 2] * imu->cov_acc[2] * R[3 * j + 2];
+                P[(12 + i) * D + 12 + j] += q * dt * dt;
+            }
+        }
+        double Rn[9];   // :355-364
+        mul33(R, Ef, Rn);
+        std::memcpy(R, Rn, sizeof(R));
+        for (int i = 0; i < 3; i++) acc_imu[i] = R[3 * i] * acc[0] + R[3 * i + 1] * acc[1] + R[3 * i + 2] * acc[2] + s->gravity[i];
+        for (int i = 0; i < 3; i++) {
+            pos[i] = pos[i] + vel[i] * dt + 0.5 * acc_imu[i] * dt * dt;
+            vel[i] = vel[i] + acc_imu[i] * dt;
+        }
+        std::memcpy(imu->angvel_last, angvel, sizeof(angvel));   // :367-370
+        std::memcpy(imu->acc_s_last, acc_imu, sizeof(acc_imu));
+        put_pose6d(poses + (size_t)out * LIINIT_POSE6D_DOUBLES, tail[0] - pcl_beg_time, acc_imu, angvel, vel, pos, R);
+        out++;
+    }
+    // extrapolation to the scan end, forwards (note = 1) or backwards (note = -1) from the last sample (:374-378)
+    const double note = pcl_end_time > imu_end_time ? 1.0 : -1.0;
+    const double dt = note * (pcl_end_time - imu_end_time);
+    const double w[3] = {note * angvel[0], note * angvel[1], note * angvel[2]};
+    double E[9];
+    so3_exp_dt(w, dt, E);
+    mul33(R, E, s->rot_end);
+    for (int i = 0; i < 3; i++) {
+        s->vel_end[i] = vel[i] + note * acc_imu[i] * dt;
+        s->pos_end[i] = pos[i] + note * vel[i] * dt + note * 0.5 * acc_imu[i] * dt * dt;
+    }
+    std::memcpy(imu->last_imu, sample(n), sizeof(imu->last_imu));   // :381-382
+    imu->last_lidar_end_time = pcl_end_time;
+    *npose = out;
+    return LIINIT_OK;
+}
+
 int liinit_fov_segment(const double* pos, double cube_len, double det_range, float* box, int* initialized, float* out) {
     const double MOV_THRESHOLD = 1.5;   // laserMapping.cpp:58
     if (!*initialized) {                 // :266-272

@@ -66,6 +66,60 @@ int liinit_scan_update(liinit_ctx* h, liinit_state* state, int max_iteration, in
  * rot_end <- rot_end Exp(bias_g dt), pos_end += vel_end dt. dt: scan-to-scan time (0.1 for the first frame, :217-223). */
 void liinit_propagate_cv(liinit_state* s, double dt, const double cov_gyr_scale[3], const double cov_acc_scale[3]);
 
+/* ---- the IMU branch of ImuProcess (src/IMU_Processing.hpp), used in LIO mode after the hand-over of LI_Initialization ---- */
+#define LIINIT_IMU_SAMPLE_DOUBLES 7   /* one IMU sample: {stamp [s], gyr xyz [rad/s], acc xyz} */
+#define LIINIT_POSE6D_DOUBLES 22      /* Pose6D (common_lib.h:184-199): {offset_time, acc[3], gyr[3], vel[3], pos[3], rot[9]} */
+
+/* The members of ImuProcess (IMU_Processing.hpp:56-89) that its IMU branch reads or writes. */
+typedef struct liinit_imu {
+    double last_imu[LIINIT_IMU_SAMPLE_DOUBLES];   /* last_imu_: last sample of the previous measure group */
+    double angvel_last[3];        /* bias-corrected mean angular velocity of the last IMU interval */
+    double acc_s_last[3];         /* world-frame acceleration of the last IMU interval */
+    double last_lidar_end_time;   /* last_lidar_end_time_: end of the previous scan */
+    double cov_acc[3];
+    double cov_gyr[3];
+    double cov_acc_scale[3];
+    double cov_gyr_scale[3];
+    double cov_R_LI[3];
+    double cov_T_LI[3];
+    double cov_bias_gyr[3];
+    double cov_bias_acc[3];
+    double mean_acc_norm;         /* IMU_mean_acc_norm: the accelerometer reading of 1 g */
+    int need_init;                /* imu_need_init_ */
+    int reserved;
+} liinit_imu;
+
+/* ImuProcess() (IMU_Processing.hpp:92-108): cov_acc = cov_gyr = 0.1, cov_R_LI = 1e-5, cov_T_LI = 1e-4, bias covariances 1e-4,
+ * angvel_last = 0, last_imu_ = a zero sample, need_init = 1. Members the constructor leaves unset get the values the node sets
+ * before first use: cov_acc_scale = cov_gyr_scale = 0.1 and mean_acc_norm = 9.81 (laserMapping.cpp:76,94). acc_s_last and
+ * last_lidar_end_time, never written before the first propagation in LI-Init, are 0. */
+void liinit_imu_init(liinit_imu* imu);
+/* The setters the node calls (laserMapping.cpp:833-838 from the YAML, :1224-1228 at the hand-over). set_gyr_cov / set_acc_cov
+ * set the scales (cov_gyr_scale / cov_acc_scale), as the reference's do. */
+void liinit_imu_set_gyr_cov(liinit_imu* imu, const double v[3]);
+void liinit_imu_set_acc_cov(liinit_imu* imu, const double v[3]);
+void liinit_imu_set_R_LI_cov(liinit_imu* imu, const double v[3]);
+void liinit_imu_set_T_LI_cov(liinit_imu* imu, const double v[3]);
+void liinit_imu_set_gyr_bias_cov(liinit_imu* imu, const double v[3]);
+void liinit_imu_set_acc_bias_cov(liinit_imu* imu, const double v[3]);
+void liinit_imu_set_mean_acc_norm(liinit_imu* imu, double mean_acc_norm);
+
+/* The switch scan, the first scan after LI_init_done (Process, IMU_Processing.hpp:445-453): records the last of the n samples as
+ * last_imu_, sets cov_acc / cov_gyr from the scales and clears need_init. Nothing is propagated and the state is not an argument:
+ * the scan reuses the previous undistorted cloud (Process returns before touching it). n = 0: nothing happens (:423). */
+int liinit_imu_switch(liinit_imu* imu, const double* samples, int n);
+
+/* The forward part of propagation_and_undist (IMU_Processing.hpp:271-382) for one measure group of n samples
+ * (n x LIINIT_IMU_SAMPLE_DOUBLES, ascending stamps): last_imu_ is put in front, pairs whose later sample is older than
+ * last_lidar_end_time are skipped, each remaining pair propagates the state (mean rate minus bias_g, mean specific force scaled
+ * by 9.81 / mean_acc_norm minus bias_a) and the covariance (cov <- F cov F^T + Q), then the state is extrapolated to the scan end
+ * pcl_beg_time + pcl_end_offset_ms / 1000 (forwards or backwards, :374-378).
+ * poses: the IMUpose table for liinit_raw_undistort_imu, room for n + 1 poses of LIINIT_POSE6D_DOUBLES; *npose its length.
+ * n = 0: nothing happens, *npose = 0 (Process returns at once, :423). LIINIT_ERR_INVALID while need_init is set (the switch scan
+ * comes first); LIINIT_ERR_CAPACITY, with nothing changed, when the table would be longer than LIINIT_MAX_IMU_POSES. */
+int liinit_imu_propagate(liinit_imu* imu, liinit_state* s, const double* samples, int n, double pcl_beg_time, double pcl_end_offset_ms,
+                         double* poses, int* npose);
+
 /* lasermap_fov_segment (laserMapping.cpp:260-305): keeps a cube_len-sized local map box around the LiDAR and, when the
  * LiDAR comes within MOV_THRESHOLD*det_range of a face, shifts the box and returns the slabs that fell out of it
  * (cub_needrm) -- the boxes to hand to liinit_map_delete_boxes. local_box: {min xyz, max xyz}, state kept by the caller;

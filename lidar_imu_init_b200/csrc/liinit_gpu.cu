@@ -115,7 +115,7 @@ struct Ctx {
     VgParams* d_vg_params = nullptr;
     int raw_n = 0;                          // raw (not yet downsampled) cloud staged in d_stage_pts, w = time [ms]
     unsigned long long* d_tmin_idx = nullptr;
-    double* d_poses = nullptr;              // IMU pose table for the undistortion (<= 4096 x 22 doubles)
+    double* d_poses = nullptr;              // IMU pose table for the undistortion (<= LIINIT_MAX_IMU_POSES x 22 doubles)
     VoxTmp V{};
     // scan
     ScanDev S{};
@@ -698,7 +698,7 @@ int liinit_create(const liinit_config* cfg, liinit_ctx** out) {
         CUC(cudaMalloc(&c->d_rs_hist, ((size_t)batch / RS_TILE + 2) * 256 * 4));
         CUC(cudaMalloc(&c->d_vg_params, sizeof(VgParams)));
         CUC(cudaMalloc(&c->d_tmin_idx, 8));
-        CUC(cudaMalloc(&c->d_poses, 4096 * LI_POSE6D_DOUBLES * sizeof(double)));
+        CUC(cudaMalloc(&c->d_poses, LIINIT_MAX_IMU_POSES * LI_POSE6D_DOUBLES * sizeof(double)));
     }
     int ns = cfg->max_scan_points + 64;   // (+ slack: equal-sized shard slots of a frame cut over up to 64 ranks)
     CUC(cudaMalloc(&c->d_acc, 160 * sizeof(double)));
@@ -1122,7 +1122,7 @@ int liinit_raw_undistort_imu(liinit_ctx* h, const double* poses, int npose, cons
     Ctx* c = &h->c;
     CU(cudaSetDevice(c->device));
     if (c->raw_n <= 0) return fail(c, LIINIT_ERR_INVALID, "no raw cloud staged (liinit_raw_upload)");
-    if (npose > 4096) return fail(c, LIINIT_ERR_CAPACITY, "IMU pose table too long");
+    if (npose > LIINIT_MAX_IMU_POSES) return fail(c, LIINIT_ERR_CAPACITY, "IMU pose table too long");
     CU(cudaMemcpyAsync(c->d_poses, poses, (size_t)npose * LI_POSE6D_DOUBLES * sizeof(double), cudaMemcpyHostToDevice, c->stream));
     PoseD S;
     fill_pose(S, rot_end, pos_end, R_LI, T_LI);
@@ -1146,6 +1146,26 @@ int liinit_raw_download(liinit_ctx* h, float* xyz, int cap, int* n) {
             xyz[3 * (size_t)i] = b[i].x; xyz[3 * (size_t)i + 1] = b[i].y; xyz[3 * (size_t)i + 2] = b[i].z;
         }
     }
+    return LIINIT_OK;
+}
+
+int liinit_raw_download_world(liinit_ctx* h, const double* R, const double* p, const double* RLI, const double* TLI, float* xyz, int cap,
+                              int* n) {
+    if (!h || !R || !p || !RLI || !TLI || !n) return LIINIT_ERR_INVALID;
+    Ctx* c = &h->c;
+    CU(cudaSetDevice(c->device));
+    if (c->raw_n <= 0) return fail(c, LIINIT_ERR_INVALID, "no raw cloud staged (liinit_raw_upload)");
+    *n = c->raw_n;
+    if (!xyz) return LIINIT_OK;
+    if (cap < c->raw_n) return fail(c, LIINIT_ERR_CAPACITY, "cap_points is smaller than the staged raw cloud");
+    PoseD P;
+    fill_pose(P, R, p, RLI, TLI);
+    // the strided staging buffer (>= 12 floats per staged point) is free once the cloud has been repacked: it holds the output
+    k_raw_to_world<<<nblk(c->raw_n, 256), 256, 0, c->stream>>>(c->d_stage_pts, c->raw_n, P, c->d_stage_raw);
+    c->launches++;
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(xyz, c->d_stage_raw, (size_t)c->raw_n * 3 * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
     return LIINIT_OK;
 }
 

@@ -97,6 +97,19 @@ __global__ void k_undistort_imu(float4* __restrict__ pts, int n, const double* _
     pts[i] = make_float4((float)w[0], (float)w[1], (float)w[2], p.w);
 }
 
+// pointBodyToWorld (laserMapping.cpp:209-220) over the staged cloud, one thread per point, packed xyz out in upload order
+// (publish_frame_world / pcd_save on feats_undistort, :560-603).
+__global__ void k_raw_to_world(const float4* __restrict__ pts, int n, PoseD P, float* __restrict__ out) {
+    int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const float4 p = pts[i];
+    float wx, wy, wz;
+    li_body_to_world(P, p.x, p.y, p.z, wx, wy, wz);
+    out[3 * (size_t)i] = wx;
+    out[3 * (size_t)i + 1] = wy;
+    out[3 * (size_t)i + 2] = wz;
+}
+
 // time range of the staged cloud: min time + its first index, max time (ordered-int atomics on non-negative floats)
 __global__ void k_time_range(const float4* __restrict__ pts, int n, unsigned long long* __restrict__ tmin_idx, int* __restrict__ tmax) {
     int i = blockIdx.x * blockDim.x + threadIdx.x;

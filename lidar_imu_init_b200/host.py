@@ -19,6 +19,19 @@ class ScanStats(C.Structure):
                 ("last_rot_deg", C.c_double), ("last_trans_cm", C.c_double), ("res_sq", C.c_double)]
 
 
+class Imu(C.Structure):
+    """struct liinit_imu: the members of ImuProcess that its IMU branch uses (csrc/host/liinit_host.h)."""
+    _fields_ = [("last_imu", C.c_double * 7), ("angvel_last", C.c_double * 3), ("acc_s_last", C.c_double * 3), ("last_lidar_end_time", C.c_double),
+                ("cov_acc", C.c_double * 3), ("cov_gyr", C.c_double * 3), ("cov_acc_scale", C.c_double * 3), ("cov_gyr_scale", C.c_double * 3),
+                ("cov_R_LI", C.c_double * 3), ("cov_T_LI", C.c_double * 3), ("cov_bias_gyr", C.c_double * 3), ("cov_bias_acc", C.c_double * 3),
+                ("mean_acc_norm", C.c_double), ("need_init", C.c_int), ("reserved", C.c_int)]
+
+
+IMU_SAMPLE_DOUBLES = 7   # {stamp, gyr xyz, acc xyz}
+POSE6D_DOUBLES = 22      # {offset_time, acc[3], gyr[3], vel[3], pos[3], rot[9]}
+MAX_IMU_POSES = 4096     # LIINIT_MAX_IMU_POSES (include/liinit_gpu.h)
+
+
 def load():
     global _LIB
     if _LIB is not None:
@@ -38,6 +51,18 @@ def load():
     L.liinit_scan_update.argtypes = [C.c_void_p, _f64, C.c_int, C.c_int, C.POINTER(ScanStats)]
     L.liinit_propagate_cv.restype = None
     L.liinit_propagate_cv.argtypes = [_f64, C.c_double, _f64, _f64]
+    pimu = C.POINTER(Imu)
+    L.liinit_imu_init.restype = None
+    L.liinit_imu_init.argtypes = [pimu]
+    for f in ("gyr_cov", "acc_cov", "R_LI_cov", "T_LI_cov", "gyr_bias_cov", "acc_bias_cov"):
+        getattr(L, "liinit_imu_set_" + f).restype = None
+        getattr(L, "liinit_imu_set_" + f).argtypes = [pimu, _f64]
+    L.liinit_imu_set_mean_acc_norm.restype = None
+    L.liinit_imu_set_mean_acc_norm.argtypes = [pimu, C.c_double]
+    L.liinit_imu_switch.restype = C.c_int
+    L.liinit_imu_switch.argtypes = [pimu, _f64, C.c_int]
+    L.liinit_imu_propagate.restype = C.c_int
+    L.liinit_imu_propagate.argtypes = [pimu, _f64, _f64, C.c_int, C.c_double, C.c_double, _f64, C.POINTER(C.c_int)]
     L.liinit_fov_segment.restype = C.c_int
     L.liinit_fov_segment.argtypes = [_f64, C.c_double, C.c_double, np.ctypeslib.ndpointer(dtype=np.float32, flags='C_CONTIGUOUS'), C.POINTER(C.c_int),
                                      np.ctypeslib.ndpointer(dtype=np.float32, flags='C_CONTIGUOUS')]
@@ -104,6 +129,46 @@ def scan_update(gpu: capi.LiInitGpu, state, max_iteration=5, imu_en=False):
     if rc != 0:
         raise capi.LiInitError(rc, (gpu.L.liinit_last_error(gpu.h) or b"").decode())
     return s, {k: getattr(st, k) for k, _ in ScanStats._fields_}
+
+
+class ImuProcess:
+    """The IMU branch of ImuProcess (IMU_Processing.hpp) over liinit_imu_*: its members live in a struct liinit_imu."""
+
+    def __init__(self):
+        self.m = Imu()
+        load().liinit_imu_init(C.byref(self.m))
+
+    def set_cov(self, which: str, v):
+        """which: gyr_cov, acc_cov (the scales), R_LI_cov, T_LI_cov, gyr_bias_cov or acc_bias_cov."""
+        v = np.full(3, v, np.float64) if np.isscalar(v) else np.ascontiguousarray(v, np.float64)
+        getattr(load(), "liinit_imu_set_" + which)(C.byref(self.m), v)
+
+    def set_mean_acc_norm(self, v: float):
+        load().liinit_imu_set_mean_acc_norm(C.byref(self.m), float(v))
+
+    @property
+    def need_init(self) -> bool:
+        return bool(self.m.need_init)
+
+    def switch(self, samples):
+        """The switch scan (Process :445-453): samples [k, 7] {stamp, gyr, acc}."""
+        a = np.ascontiguousarray(samples, np.float64).reshape(-1, IMU_SAMPLE_DOUBLES)
+        rc = load().liinit_imu_switch(C.byref(self.m), a.reshape(-1), len(a))
+        if rc != 0:
+            raise capi.LiInitError(rc, "liinit_imu_switch")
+
+    def propagate(self, state, samples, pcl_beg_time: float, pcl_end_offset_ms: float):
+        """propagation_and_undist without its point loop: returns (propagated state, IMUpose table [npose, 22])."""
+        s = np.ascontiguousarray(state, np.float64).copy()
+        a = np.ascontiguousarray(samples, np.float64).reshape(-1, IMU_SAMPLE_DOUBLES)
+        poses = np.zeros((len(a) + 1, POSE6D_DOUBLES))
+        n = C.c_int(0)
+        rc = load().liinit_imu_propagate(C.byref(self.m), s, a.reshape(-1), len(a), float(pcl_beg_time), float(pcl_end_offset_ms), poses.reshape(-1),
+                                         C.byref(n))
+        if rc != 0:
+            raise capi.LiInitError(rc, "liinit_imu_propagate: " + ("IMU pose table longer than %d poses" % MAX_IMU_POSES if rc == -3 else
+                                                                   "called before the switch scan"))
+        return s, poses[:n.value]
 
 
 class FovSegmenter:

@@ -1,11 +1,18 @@
-"""The LiDAR-only branch of the node's main loop (src/laserMapping.cpp:893-1234) over the C-ABI: per scan
-constant-velocity propagation -> ICP / IESKF update on the device map -> map_incremental -> LI-Init data accumulation.
+"""The node's main loop (src/laserMapping.cpp:893-1234) over the C-ABI.
 
-Host-side mirror used by the replay tool and the end-to-end test; every step is one call into the native libraries
-(libliinit_host.so: liinit_propagate_cv, liinit_scan_update; libliinit_gpu.so: liinit_scan_upload / liinit_map_*;
-libliinit_calib.so: li_calib_*). Nothing is computed in Python.
+process_scan: the LiDAR-only branch on a downsampled, undistorted scan -- constant-velocity propagation -> ICP / IESKF update on
+the device map -> map_incremental -> LI-Init data accumulation.
+process_raw: the whole loop body on a raw, timed scan, in both modes -- LiDAR-only (constant-velocity propagation, device
+undistortion) and, after the hand-over of LI_Initialization, LIO (IMU propagation, device undistortion from the IMU pose table);
+then the device voxel grid, the update and map_incremental.
+
+Host-side mirror used by the replay tool and the end-to-end tests; every step is one call into the native libraries
+(libliinit_host.so: liinit_propagate_cv, liinit_imu_*, liinit_scan_update; libliinit_gpu.so: liinit_raw_* / liinit_scan_upload /
+liinit_map_*; libliinit_calib.so: li_calib_*). Nothing is computed in Python.
 """
 from __future__ import annotations
+
+from collections import deque
 
 import numpy as np
 
@@ -13,9 +20,52 @@ from . import capi, host
 from .calib import LiCalib
 
 
+class ImuBuffer:
+    """The node's imu_buffer: imu_cbk's time compensation (laserMapping.cpp:412-423) and sync_packages's selection of a measure
+    group (:466-474). Rows are {stamp, gyr xyz, acc xyz}."""
+
+    def __init__(self, timediff_imu_wrt_lidar: float = 0.0):
+        self.timediff = float(timediff_imu_wrt_lidar)
+        self.time_lag = 0.0             # time_lag_IMU_wtr_lidar, set at the hand-over
+        self.last_stamp = -np.inf       # last_timestamp_imu
+        self.rows = deque()
+
+    def push(self, t, gyr, acc):
+        stamp = float(t) - self.timediff - self.time_lag
+        if stamp < self.last_stamp:     # "IMU loop back, clear IMU buffer" (:415-419)
+            self.rows.clear()
+        self.last_stamp = stamp
+        self.rows.append(np.concatenate([[stamp], np.asarray(gyr, float), np.asarray(acc, float)]))
+
+    def ready(self, lidar_end_time: float) -> bool:
+        """sync_packages waits until an IMU sample at or after the scan end has arrived (:461-462)."""
+        return self.last_stamp >= lidar_end_time
+
+    def pop(self, lidar_end_time: float) -> np.ndarray:
+        """The measure group of a scan ending at lidar_end_time: the buffered samples with stamp <= lidar_end_time (:466-474)."""
+        out = []
+        imu_time = self.rows[0][0] if self.rows else 0.0
+        while self.rows and imu_time < lidar_end_time:
+            imu_time = self.rows[0][0]
+            if imu_time > lidar_end_time:
+                break
+            out.append(self.rows.popleft())
+        return np.array(out, float).reshape(-1, 7)
+
+    def shift(self, time_lag: float):
+        """The hand-over (:1217-1220): the buffered stamps and every later one are moved by -time_lag. (Later samples are compared
+        against the last stamp before the shift, so the first one after it clears the buffer when the lag exceeds a sample period,
+        as imu_cbk does.)"""
+        self.time_lag = float(time_lag)
+        for r in self.rows:
+            r[0] -= self.time_lag
+
+
 class LidarOdometry:
     def __init__(self, gpu: capi.LiInitGpu, filter_size_map: float, max_iteration: int = 4, gyr_cov: float = 0.1, acc_cov: float = 0.1,
-                 orig_odom_freq: int = 10, cut_frame_num: int = 1, data_accum_length: float = 300.0, calib: LiCalib | None = None):
+                 orig_odom_freq: int = 10, cut_frame_num: int = 1, data_accum_length: float = 300.0, calib: LiCalib | None = None,
+                 filter_size_surf: float | None = None, rot_LI_cov: float = 0.00005, trans_LI_cov: float = 0.0005, b_gyr_cov: float = 0.0001,
+                 b_acc_cov: float = 0.0001, mean_acc_norm: float = 9.81):
         self.g = gpu
         self.ds = float(filter_size_map)
         self.max_iteration = int(max_iteration)            # "max_iteration", laserMapping.cpp:767
@@ -32,6 +82,17 @@ class LidarOdometry:
         self.move_start_time = 0.0
         self.stats = None
         self.imu_en = False
+        # process_raw: the voxel-grid leaf of the scan (mapping/filter_size_surf, :772), the IMU buffer and the IMU processor
+        # configured as the node does it at start-up (:833-838)
+        self.filter_size_surf = self.ds if filter_size_surf is None else float(filter_size_surf)
+        self.mean_acc_norm = float(mean_acc_norm)
+        self.imu_buffer = ImuBuffer()
+        self.imu_proc = self._make_imu_proc()
+        for which, v in (("gyr_cov", gyr_cov), ("acc_cov", acc_cov), ("R_LI_cov", rot_LI_cov), ("T_LI_cov", trans_LI_cov),
+                         ("gyr_bias_cov", b_gyr_cov), ("acc_bias_cov", b_acc_cov)):
+            self.imu_proc.set_cov(which, v)
+        self.lidar_end_time = None
+        self.switch_scan = None   # index (frame_num) of the scan that switched to LIO mode
 
     def push_imu(self, omg, acc, t, mean_acc_norm=9.81):
         """imu_cbk in LO mode (:428-430)."""
@@ -69,7 +130,68 @@ class LidarOdometry:
             self.data_accum_finished = ok
         return self.state
 
-    # the three calls into the hot path; a test substitutes the CPU oracle here to drive the SAME loop from the other side
+    def process_raw(self, raw_pts12: np.ndarray, t_beg: float, imu_group: np.ndarray | None = None):
+        """One pass of the loop body (laserMapping.cpp:893-1160) for a raw scan: raw_pts12 [n, 12] float32 in the PointType layout
+        with the per-point time offset in ms in the curvature field (index 9), t_beg = lidar_beg_time. imu_group [k, 7] {stamp, gyr,
+        acc}: the measure group; None -> the samples of imu_buffer with stamp <= lidar_end_time (sync_packages, :466-474).
+        Returns the posterior state.
+
+        LiDAR-only mode: constant-velocity propagation, device undistortion with omega = bias_g. LIO mode: IMU propagation, device
+        undistortion from the IMU pose table. The first scan after the hand-over only switches the IMU processor: like Process, it
+        neither propagates nor touches the undistorted cloud, so the cloud of the previous scan -- still staged on the device -- is
+        downsampled and matched again (the reference keeps feats_undistort, :909-918)."""
+        raw = np.ascontiguousarray(raw_pts12, np.float32)
+        end_ms = float(raw[:, 9].max())                     # points.back().curvature of the time-sorted cloud
+        t_end = t_beg + end_ms / 1000.0                     # lidar_end_time (:455-456)
+        group = self.imu_buffer.pop(t_end) if imu_group is None else np.asarray(imu_group, float).reshape(-1, 7)
+        if not self.imu_en:
+            # Forward_propagation_without_imu (IMU_Processing.hpp:204-267)
+            if self.first_prop:
+                dt = 0.1
+                self.first_prop = False
+            else:
+                dt = t_beg - self.t_last
+            self.t_last = t_beg
+            self.state = host.propagate_cv(self.state, dt, self.gyr_cov, self.acc_cov)
+            self._undistort_cv(raw, self.state)
+        elif len(group) and not self.imu_proc.need_init:
+            self.state, poses = self._propagate_imu(self.state, group, t_beg, end_ms)   # propagation_and_undist (:269-416)
+            self._undistort_imu(raw, poses, self.state)
+        elif len(group):
+            self.imu_proc.switch(group)                     # Process, IMU_Processing.hpp:445-453: no propagation, cloud kept
+            self.switch_scan = self.frame_num
+        # (an empty group in LIO mode: Process returns at once, :423 -- nothing propagated, cloud kept)
+        self._downsample(self.filter_size_surf)             # downSizeFilterSurf (:917-918)
+        self.lidar_end_time = t_end
+        if not self.map_ready:                              # :921-931
+            body = self._scan_body()
+            if len(body) > 5:
+                R, p, RLI, TLI = host.state_pose(self.state)
+                world = (R @ (RLI @ body.T.astype(np.float64) + TLI[:, None]) + p[:, None]).T.astype(np.float32)
+                self._map_build(world)
+                self.map_ready = True
+            return self.state
+        self.state, self.stats = self._scan_update_resident(self.state)   # :936-1134
+        R, p, RLI, TLI = host.state_pose(self.state)
+        self._map_incremental(R, p, RLI, TLI)               # :1140
+        if not self.imu_en and not self.data_accum_start and np.linalg.norm(p) > 0.05:   # :1145-1149
+            self.data_accum_start = True
+            self.move_start_time = t_end
+        self.frame_num += 1                                 # :1160
+        if not self.imu_en and not self.data_accum_finished and self.data_accum_start:   # :1190-1196
+            bias_g, vel = self.state[27:30], self.state[24:27]
+            self.calib.push_lidar(R, bias_g, vel, t_end)
+            ok, _ = self.calib.data_sufficiency(self.frame_num, bias_g, self.orig_odom_freq, self.cut_frame_num)
+            self.data_accum_finished = ok
+        return self.state
+
+    def world_cloud(self):
+        """The undistorted raw cloud of the last process_raw in the world frame with the current state (publish_frame_world with
+        dense_publish_en, pcd_save; laserMapping.cpp:560-603), [n, 3] float32 in upload order."""
+        R, p, RLI, TLI = host.state_pose(self.state)
+        return self.g.raw_world(R, p, RLI, TLI)
+
+    # the calls into the hot path; a test substitutes the CPU oracle here to drive the SAME loop from the other side
     def _map_build(self, world):
         self.g.map_build(world)
 
@@ -79,6 +201,32 @@ class LidarOdometry:
 
     def _map_incremental(self, R, p, RLI, TLI):
         self.g.map_incremental(R, p, RLI, TLI, self.ds)
+
+    # process_raw's stages
+    def _make_imu_proc(self):
+        return host.ImuProcess()
+
+    def _propagate_imu(self, state, group, t_beg, end_ms):
+        return self.imu_proc.propagate(state, group, t_beg, end_ms)
+
+    def _undistort_cv(self, raw, state):
+        self.g.raw_upload(raw, 9)
+        self.g.raw_undistort_cv(state[27:30], state[0:9], state[24:27])   # omega = bias_g, rot_end / vel_end propagated
+
+    def _undistort_imu(self, raw, poses, state):
+        self.g.raw_upload(raw, 9)
+        if len(poses) >= 2:   # (one pose: the back-propagation loop of the reference runs zero times)
+            R, p, RLI, TLI = host.state_pose(state)
+            self.g.raw_undistort_imu(poses, R, p, RLI, TLI)
+
+    def _downsample(self, leaf):
+        self.g.raw_downsample(leaf)
+
+    def _scan_body(self):
+        return self.g.scan_body()
+
+    def _scan_update_resident(self, state):
+        return host.scan_update(self.g, state, self.max_iteration, self.imu_en)
 
     def hand_over(self, res):
         """laserMapping.cpp:1198-1222 after LI_Initialization: the pose is re-expressed in the IMU frame with the calibrated extrinsic,
@@ -94,6 +242,11 @@ class LidarOdometry:
         s[27:30] = np.asarray(res["gyro_bias"], float)      # bias_g (:1209)
         s[30:33] = np.asarray(res["acc_bias"], float)       # bias_a (:1210)
         self.imu_en = True
+        # (:1217-1228) the buffered IMU stamps move by the total time lag; the IMU processor switches at its next scan
+        self.imu_buffer.shift(float(res["time_lag_1"]) + float(res["time_lag_2"]))
+        self.imu_proc.set_mean_acc_norm(self.mean_acc_norm)
+        for which, v in (("gyr_cov", 0.1), ("acc_cov", 0.1), ("gyr_bias_cov", 0.0001), ("acc_bias_cov", 0.0001)):
+            self.imu_proc.set_cov(which, v)
 
     def initialize(self, timediff_imu_wrt_lidar: float = 0.0):
         """LI_Initialization on what has been accumulated (:1198); returns the calibration dict of calib.LiCalib."""

@@ -238,6 +238,56 @@ def scan_points(scene: Scene, pose: Pose, N: int, seed: int = 2, det_range: floa
     return np.ascontiguousarray(Pb, dtype=np.float32)
 
 
+def timed_scan_points(scene: Scene, pose_at, t_beg: float, dur: float, N: int, seed: int = 2, det_range: float = 450.0,
+                      blind: float = 2.0, sigma: float = 0.01) -> np.ndarray:
+    """N raw points of a moving LiDAR as the driver delivers them: float32 [N, 12] in the pcl::PointXYZINormal layout
+    (x, y, z at 0:3, intensity at 8, curvature at 9), ascending in time.
+
+    Every point gets a time t uniform in [t_beg, t_beg + dur] and is expressed in the LiDAR frame of the pose at t.
+    curvature = (t - t_beg) in milliseconds, the per-point offset the undistortion reads (src/preprocess.cpp).
+    pose_at(t) -> (R [n,3,3], p [n,3]): the LiDAR frame's orientation and origin in the world at the times t [n].
+    Surface sampling, range gate and range noise as in scan_points."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    areas = np.array([r.area for r in scene.rects])
+    cdf = np.cumsum(areas) / areas.sum()
+    O_all = np.stack([r.o for r in scene.rects])
+    U_all = np.stack([r.u * r.a for r in scene.rects])
+    V_all = np.stack([r.v * r.b for r in scene.rects])
+    got_p, got_t = [], []
+    need = N
+    guard = 0
+    while need > 0:
+        guard += 1
+        if guard > 200:
+            raise RuntimeError("could not sample enough in-range surface points")
+        k = int(need * 1.3) + 16
+        t = t_beg + dur * rng.uniform(size=k)
+        R, sensor = pose_at(t)
+        ri = np.searchsorted(cdf, rng.uniform(size=k))
+        s = rng.uniform(size=k)
+        u = rng.uniform(size=k)
+        P = O_all[ri] + s[:, None] * U_all[ri] + u[:, None] * V_all[ri]
+        d = np.linalg.norm(P - sensor, axis=1)
+        ok = (d > blind) & (d < det_range)
+        if sigma > 0:
+            ray = (P - sensor) / d[:, None]
+            P = P + ray * rng.normal(0.0, sigma, k)[:, None]
+        # world -> LiDAR frame at the point's own time: R^T (p_w - p)
+        B = np.einsum("nji,nj->ni", R[ok], P[ok] - sensor[ok])
+        got_p.append(B[:need])
+        got_t.append(t[ok][:need])
+        need -= len(got_p[-1])
+    B = np.concatenate(got_p, 0)
+    t = np.concatenate(got_t, 0)
+    o = np.argsort(t, kind="stable")
+    out = np.zeros((N, 12), np.float32)
+    out[:, 0:3] = B[o]
+    out[:, 3] = 1.0
+    out[:, 8] = rng.uniform(0.0, 255.0, N)
+    out[:, 9] = (t[o] - t_beg) * 1000.0
+    return out
+
+
 def default_sensor_pose(scene: Scene, R_LI=None, T_LI=None, yaw_deg: float = 20.0) -> Pose:
     """Ground-truth pose: sensor 1.5 m above the floor near the scene centre, mild attitude."""
     if R_LI is None:
