@@ -108,6 +108,51 @@ int liinit_raw_undistort_cv(liinit_ctx* h, const double omega[3], const double r
 #define LIINIT_MAX_IMU_POSES 4096
 int liinit_raw_undistort_imu(liinit_ctx* h, const double* poses, int npose, const double rot_end[9], const double pos_end[3],
                              const double R_LI[9], const double T_LI[3]);
+/* ---- cut-frame preprocess (Preprocess::process_cut_frame_livox / _pcl2, src/preprocess.cpp:50-335): one driver message ->
+ * decoded, filtered, time-sorted, cut and re-timed sub-frames, kept on the device. A cut writes one of LIINIT_FRAME_SLOTS message
+ * slots (round robin); each returned sub-frame carries a handle that liinit_frame_stage turns into the staged raw cloud, exactly as
+ * liinit_raw_upload(pts12, 12, 9, n) of the same points would. A message that yields no sub-frame does not take a slot. The buffers
+ * are allocated on the first cut. Errors: LIINIT_ERR_CAPACITY when n exceeds the raw staging capacity (max(max_scan_points, 2^20))
+ * or required_cut_num exceeds cap; LIINIT_ERR_INVALID for a bad lidar_type / point_filter_num / required_frame_num / layout, or
+ * (spinning sensors whose offset times come from the rotation model) a ring >= 128. Every error leaves the context as it was. */
+#define LIINIT_FRAME_SLOTS 4
+#define LIINIT_FRAME_MAX_CUT 256     /* largest required_frame_num */
+#define LIINIT_LIDAR_AVIA 1          /* Livox CustomMsg (preprocess.h LID_TYPE) */
+#define LIINIT_LIDAR_VELO 2          /* PointCloud2: velodyne_ros::Point {x,y,z,intensity f32, time f32, ring u16} */
+#define LIINIT_LIDAR_OUSTER 3        /* ouster_ros::Point {.., intensity f32, t u32, ring u8} */
+#define LIINIT_LIDAR_PANDAR 5        /* pandar_ros::Point {.., intensity f32, timestamp f64, ring u16} */
+#define LIINIT_LIDAR_ROBOSENSE 6     /* robosense_ros::Point {.., intensity u8, ring u16, timestamp f64} */
+typedef struct liinit_frame_params {
+    int lidar_type;          /* preprocess/lidar_type */
+    int N_SCANS;             /* preprocess/scan_line */
+    double blind;            /* preprocess/blind [m] */
+    int point_filter_num;    /* point_filter_num */
+    int required_frame_num;  /* cut_frame_num: sub-frames per message once scan_count passes 5 (Livox) / 20 (PointCloud2) */
+    int scan_count;          /* the node's scan_count for this message (incremented before the cut, laserMapping.cpp:317,355) */
+    double stamp;            /* msg->header.stamp.toSec() [s] */
+} liinit_frame_params;
+typedef struct liinit_pcl2_layout {
+    int point_step;          /* bytes per point */
+    int off_x, off_y, off_z, off_intensity, off_time, off_ring;   /* byte offsets of the fields; -1 = absent (reads as 0) */
+} liinit_pcl2_layout;
+typedef struct liinit_subframe {
+    long long handle;        /* for liinit_frame_stage / liinit_frame_download */
+    double t_beg;            /* time_buffer entry: last_frame_end_time / 1000 [s] */
+    float end_ms;            /* curvature of the last point [ms]; lidar_end_time = t_beg + end_ms / 1000 */
+    int n;                   /* points */
+} liinit_subframe;
+/* pts: n Livox CustomPoint records {u32 offset_time [ns]; f32 x, y, z; u8 reflectivity, tag, line}, stride_bytes >= 19 apart
+ * (19 on the wire, 20 as the ROS struct). out[0 .. *n_sub) receives the sub-frames in time order (0 or required_cut_num of them). */
+int liinit_frame_cut_livox(liinit_ctx* h, const void* pts, int stride_bytes, int n, const liinit_frame_params* p, liinit_subframe* out,
+                           int cap, int* n_sub);
+/* data: the PointCloud2 data buffer (little endian), n = width * height points of layout->point_step bytes. */
+int liinit_frame_cut_pcl2(liinit_ctx* h, const void* data, const liinit_pcl2_layout* layout, int n, const liinit_frame_params* p,
+                          liinit_subframe* out, int cap, int* n_sub);
+/* The sub-frame becomes the staged raw cloud (time = re-timed curvature). LIINIT_ERR_INVALID when its slot has been reused. */
+int liinit_frame_stage(liinit_ctx* h, long long handle);
+/* The sub-frame in the 12-float PointType layout: x, y, z, 1, normals 0, intensity, curvature, 0, 0. *n = its size; pts12 may
+ * be NULL to ask for it; LIINIT_ERR_CAPACITY when cap_points < *n (nothing written). */
+int liinit_frame_download(liinit_ctx* h, long long handle, float* pts12, int cap_points, int* n);
 /* The staged raw cloud as packed xyz (after whatever undistortion ran). */
 int liinit_raw_download(liinit_ctx* h, float* xyz, int cap_points, int* n);
 /* The staged (undistorted) raw cloud in the world frame, packed xyz in upload order: pointBodyToWorld (laserMapping.cpp:209-220)

@@ -27,6 +27,25 @@ class Config(C.Structure):
                 ("brick_cells_log2", C.c_int), ("hash_capacity_log2", C.c_int), ("knn_group_lanes", C.c_int), ("knn_seed_radius_cells", C.c_float), ("knn_index", C.c_int), ("reserved", C.c_int * 6)]
 
 
+class FrameParams(C.Structure):   # liinit_frame_params
+    _fields_ = [("lidar_type", C.c_int), ("N_SCANS", C.c_int), ("blind", C.c_double), ("point_filter_num", C.c_int), ("required_frame_num", C.c_int),
+                ("scan_count", C.c_int), ("stamp", C.c_double)]
+
+
+class Pcl2Layout(C.Structure):   # liinit_pcl2_layout
+    _fields_ = [("point_step", C.c_int), ("off_x", C.c_int), ("off_y", C.c_int), ("off_z", C.c_int), ("off_intensity", C.c_int), ("off_time", C.c_int),
+                ("off_ring", C.c_int)]
+
+
+class SubFrame(C.Structure):   # liinit_subframe
+    _fields_ = [("handle", C.c_longlong), ("t_beg", C.c_double), ("end_ms", C.c_float), ("n", C.c_int)]
+
+
+FRAME_MAX_CUT = 256   # LIINIT_FRAME_MAX_CUT
+# Livox CustomPoint: 19 bytes on the wire, 20 as the ROS struct (align=True)
+LIVOX_POINT = np.dtype([("offset_time", "<u4"), ("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("reflectivity", "u1"), ("tag", "u1"), ("line", "u1")])
+LIVOX_POINT_ALIGNED = np.dtype(LIVOX_POINT, align=True)
+
 _f32 = np.ctypeslib.ndpointer(dtype=np.float32, flags="C_CONTIGUOUS")
 _f64 = np.ctypeslib.ndpointer(dtype=np.float64, flags="C_CONTIGUOUS")
 _i32 = np.ctypeslib.ndpointer(dtype=np.int32, flags="C_CONTIGUOUS")
@@ -35,6 +54,7 @@ SYMBOLS = [
     "liinit_create", "liinit_destroy", "liinit_last_error", "liinit_set_stream", "liinit_map_build", "liinit_map_add_points", "liinit_map_delete_boxes",
     "liinit_map_compact", "liinit_map_validnum", "liinit_map_size", "liinit_map_download", "liinit_map_nearest_search", "liinit_scan_upload", "liinit_scan_attach_host", "liinit_scan_upload_raw", "liinit_scan_download_body", "liinit_raw_upload", "liinit_raw_undistort_cv", "liinit_raw_undistort_imu",
     "liinit_raw_download", "liinit_raw_download_world", "liinit_raw_downsample",
+    "liinit_frame_cut_livox", "liinit_frame_cut_pcl2", "liinit_frame_stage", "liinit_frame_download",
     "liinit_icp_iterate", "liinit_icp_iterate_device", "liinit_scan_download_effect", "liinit_scan_download_state",
     "liinit_map_incremental", "liinit_last_pass_timing", "liinit_last_pass_kernel_times", "liinit_launch_count", "liinit_map_stats", "liinit_knn_index",
     "liinit_comm_unique_id", "liinit_comm_init", "liinit_comm_info", "liinit_comm_last_local", "liinit_comm_mode", "liinit_debug_esti_plane", "liinit_set_reseed",
@@ -79,6 +99,11 @@ def load():
     L.liinit_raw_download.argtypes = [vp, vp, C.c_int, C.POINTER(C.c_int)]
     L.liinit_raw_download_world.argtypes = [vp, _f64, _f64, _f64, _f64, vp, C.c_int, C.POINTER(C.c_int)]
     L.liinit_raw_downsample.argtypes = [vp, C.c_float, C.POINTER(C.c_int)]
+    L.liinit_frame_cut_livox.argtypes = [vp, vp, C.c_int, C.c_int, C.POINTER(FrameParams), C.POINTER(SubFrame), C.c_int, C.POINTER(C.c_int)]
+    L.liinit_frame_cut_pcl2.argtypes = [vp, vp, C.POINTER(Pcl2Layout), C.c_int, C.POINTER(FrameParams), C.POINTER(SubFrame), C.c_int,
+                                        C.POINTER(C.c_int)]
+    L.liinit_frame_stage.argtypes = [vp, C.c_longlong]
+    L.liinit_frame_download.argtypes = [vp, C.c_longlong, vp, C.c_int, C.POINTER(C.c_int)]
     L.liinit_scan_download_body.argtypes = [vp, vp, C.c_int, C.POINTER(C.c_int)]
     L.liinit_icp_iterate.argtypes = [vp, _f64, _f64, _f64, _f64, C.c_int, C.c_int, _f64, _f64, C.POINTER(C.c_int), C.POINTER(C.c_double)]
     L.liinit_icp_iterate_device.argtypes = [vp, _f64, _f64, _f64, _f64, C.c_int, C.c_int, vp]
@@ -253,6 +278,57 @@ class LiInitGpu:
         self._ck(self.L.liinit_raw_downsample(self.h, float(leaf_size), C.byref(nd)))
         self.scan_n = nd.value
         return nd.value
+
+    # ---- cut-frame preprocess: driver message -> sub-frames on the device ----
+    def frame_cut_livox(self, points, lidar_type=1, N_SCANS=6, blind=0.01, point_filter_num=1, required_frame_num=1, scan_count=0,
+                        stamp=0.0):
+        """Preprocess::process_cut_frame_livox. points: a structured array of LIVOX_POINT (19 bytes) or LIVOX_POINT_ALIGNED (20 bytes)
+        records. Returns a list of dicts {handle, t_beg, end_ms, n}, in time order."""
+        a = np.ascontiguousarray(points)
+        stride, n = a.dtype.itemsize, len(a)
+        P = FrameParams(lidar_type, N_SCANS, blind, point_filter_num, required_frame_num, scan_count, stamp)
+        out = (SubFrame * max(required_frame_num, 1))()
+        k = C.c_int(0)
+        self._ck(self.L.liinit_frame_cut_livox(self.h, _ptr(a), stride, n, C.byref(P), out, len(out), C.byref(k)))
+        return [dict(handle=out[i].handle, t_beg=out[i].t_beg, end_ms=out[i].end_ms, n=out[i].n) for i in range(k.value)]
+
+    def frame_cut_pcl2(self, data, layout, n, lidar_type, N_SCANS=16, blind=0.01, point_filter_num=1, required_frame_num=1, scan_count=0,
+                       stamp=0.0):
+        """Preprocess::process_cut_frame_pcl2. data: the PointCloud2 data buffer (bytes or uint8 array); layout: dict of point_step and
+        the byte offsets off_x, off_y, off_z, off_intensity, off_time, off_ring (-1 or missing = absent)."""
+        a = np.ascontiguousarray(np.frombuffer(data, np.uint8) if isinstance(data, (bytes, bytearray, memoryview)) else data).view(np.uint8)
+        if a.nbytes < int(n) * int(layout["point_step"]):
+            raise ValueError(f"data holds {a.nbytes} bytes, fewer than n * point_step = {int(n) * int(layout['point_step'])}")
+        Lo = Pcl2Layout(layout["point_step"], *[int(layout.get(f, -1)) for f in ("off_x", "off_y", "off_z", "off_intensity", "off_time", "off_ring")])
+        P = FrameParams(lidar_type, N_SCANS, blind, point_filter_num, required_frame_num, scan_count, stamp)
+        out = (SubFrame * max(required_frame_num, 1))()
+        k = C.c_int(0)
+        self._ck(self.L.liinit_frame_cut_pcl2(self.h, _ptr(a), C.byref(Lo), int(n), C.byref(P), out, len(out), C.byref(k)))
+        return [dict(handle=out[i].handle, t_beg=out[i].t_beg, end_ms=out[i].end_ms, n=out[i].n) for i in range(k.value)]
+
+    def frame_stage(self, handle: int):
+        """The sub-frame becomes the staged raw cloud, as raw_upload(its PointType points, 9) would leave it."""
+        self._ck(self.L.liinit_frame_stage(self.h, int(handle)))
+        n = C.c_int(0)
+        self._ck(self.L.liinit_frame_download(self.h, int(handle), None, 0, C.byref(n)))
+        self.raw_n = n.value
+
+    def frame_size(self, handle: int):
+        """Points of a sub-frame the device still holds; None when its message slot has been reused by a later cut."""
+        n = C.c_int(0)
+        rc = self.L.liinit_frame_download(self.h, int(handle), None, 0, C.byref(n))
+        if rc == -1:
+            return None
+        self._ck(rc)
+        return n.value
+
+    def frame_download(self, handle: int):
+        """The sub-frame as [n, 12] float32 PointType rows (x, y, z, 1, normals 0, intensity, curvature, 0, 0)."""
+        n = C.c_int(0)
+        self._ck(self.L.liinit_frame_download(self.h, int(handle), None, 0, C.byref(n)))
+        out = np.zeros((n.value, 12), np.float32)
+        self._ck(self.L.liinit_frame_download(self.h, int(handle), _ptr(out), n.value, C.byref(n)))
+        return out
 
     def scan_body(self):
         n = C.c_int(0)

@@ -11,6 +11,7 @@
 #endif
 
 #include <cmath>
+#include <cstddef>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -24,6 +25,7 @@
 #include "map_kernels.cuh"
 #include "voxelgrid_kernels.cuh"
 #include "undistort_kernels.cuh"
+#include "preprocess_kernels.cuh"
 
 #ifndef LI_CELLS_MINB
 #define LI_CELLS_MINB 6
@@ -117,6 +119,27 @@ struct Ctx {
     unsigned long long* d_tmin_idx = nullptr;
     double* d_poses = nullptr;              // IMU pose table for the undistortion (<= LIINIT_MAX_IMU_POSES x 22 doubles)
     VoxTmp V{};
+    // cut-frame preprocess (liinit_frame_*), allocated on the first cut
+    bool fr_ready = false;
+    unsigned char* d_fr_in = nullptr;   // the message as received
+    size_t fr_in_bytes = 0;
+    float4* d_fr_dec = nullptr;         // decoded points by raw index: x, y, z, time [ms]
+    float* d_fr_inten = nullptr;
+    int* d_fr_flag = nullptr;
+    unsigned* d_fr_keys = nullptr;      // (sort key, raw index) pairs; d_rs_keys / d_rs_vals are the other half of the ping-pong
+    unsigned* d_fr_vals = nullptr;
+    unsigned* d_fr_aux = nullptr;       // rotation model: ring by raw index, then base time by ring-sorted position
+    double* d_fr_yaw = nullptr;         // rotation model: yaw [deg] by ring-sorted position
+    int* d_fr_tsum = nullptr;           // two arrays of per-block counts
+    int* d_fr_ring = nullptr;           // rotation model: [256] first position per ring, [256] first descent, [1] survivors
+    FrameTable* d_fr_tab = nullptr;
+    FrameTable* h_fr_tab = nullptr;     // pinned
+    float4* d_fr_slot_pts = nullptr;    // LIINIT_FRAME_SLOTS x stage_pts_cap re-timed, sorted points (sorted index j at j - 1)
+    float* d_fr_slot_inten = nullptr;
+    long long fr_seq = 0;               // cuts that produced sub-frames; message fr_seq goes to slot fr_seq % LIINIT_FRAME_SLOTS
+    long long fr_slot_seq[LIINIT_FRAME_SLOTS] = {};   // message held by each slot (-1: none; set when the buffers are allocated)
+    int fr_slot_nsub[LIINIT_FRAME_SLOTS] = {};
+    FrameSub fr_slot_sub[LIINIT_FRAME_SLOTS][LIINIT_FRAME_MAX_CUT];
     // scan
     ScanDev S{};
     float4* d_body = nullptr;
@@ -536,6 +559,125 @@ int gather_scan_state(Ctx* c) {
     return LIINIT_OK;
 }
 
+// ---- cut-frame preprocess ------------------------------------------------------------------------------------------------
+void frame_free(Ctx* c) {
+    cudaFree(c->d_fr_in); cudaFree(c->d_fr_dec); cudaFree(c->d_fr_inten); cudaFree(c->d_fr_flag); cudaFree(c->d_fr_keys); cudaFree(c->d_fr_vals);
+    cudaFree(c->d_fr_aux); cudaFree(c->d_fr_yaw); cudaFree(c->d_fr_tsum); cudaFree(c->d_fr_ring); cudaFree(c->d_fr_tab); cudaFreeHost(c->h_fr_tab);
+    cudaFree(c->d_fr_slot_pts); cudaFree(c->d_fr_slot_inten);
+    c->d_fr_in = nullptr; c->d_fr_dec = nullptr; c->d_fr_inten = nullptr; c->d_fr_flag = nullptr; c->d_fr_keys = nullptr; c->d_fr_vals = nullptr;
+    c->d_fr_aux = nullptr; c->d_fr_yaw = nullptr; c->d_fr_tsum = nullptr; c->d_fr_ring = nullptr; c->d_fr_tab = nullptr; c->h_fr_tab = nullptr;
+    c->d_fr_slot_pts = nullptr; c->d_fr_slot_inten = nullptr;
+    c->fr_in_bytes = 0;
+    c->fr_ready = false;
+}
+
+int frame_tiles(Ctx* c) { return nblk(c->stage_pts_cap, LI_FR_TILE); }
+
+// buffers of the cut, sized for stage_pts_cap points (the input buffer grows with the largest message seen)
+int frame_alloc(Ctx* c, size_t in_bytes) {
+    if (!c->fr_ready) {
+        const size_t cap = (size_t)c->stage_pts_cap;
+        cudaError_t e = cudaSuccess;
+        auto A = [&](void** p, size_t bytes) { if (e == cudaSuccess) e = cudaMalloc(p, bytes); };
+        A((void**)&c->d_fr_dec, cap * sizeof(float4));
+        A((void**)&c->d_fr_inten, cap * sizeof(float));
+        A((void**)&c->d_fr_flag, cap * sizeof(int));
+        A((void**)&c->d_fr_keys, cap * sizeof(unsigned));
+        A((void**)&c->d_fr_vals, cap * sizeof(unsigned));
+        A((void**)&c->d_fr_aux, cap * sizeof(unsigned));
+        A((void**)&c->d_fr_yaw, cap * sizeof(double));
+        A((void**)&c->d_fr_tsum, (size_t)2 * frame_tiles(c) * sizeof(int));
+        A((void**)&c->d_fr_ring, 513 * sizeof(int));
+        A((void**)&c->d_fr_tab, sizeof(FrameTable));
+        A((void**)&c->d_fr_slot_pts, LIINIT_FRAME_SLOTS * cap * sizeof(float4));
+        A((void**)&c->d_fr_slot_inten, LIINIT_FRAME_SLOTS * cap * sizeof(float));
+        if (e == cudaSuccess) e = cudaMallocHost((void**)&c->h_fr_tab, sizeof(FrameTable));
+        if (e != cudaSuccess) {
+            frame_free(c);
+            c->err = std::string("frame buffers: ") + cudaGetErrorString(e);
+            return LIINIT_ERR_CUDA;
+        }
+        for (int s = 0; s < LIINIT_FRAME_SLOTS; s++) {
+            c->fr_slot_seq[s] = -1;
+            c->fr_slot_nsub[s] = 0;
+        }
+        c->fr_ready = true;
+    }
+    if (in_bytes > c->fr_in_bytes) {
+        CU(cudaStreamSynchronize(c->stream));
+        cudaFree(c->d_fr_in);
+        c->d_fr_in = nullptr;
+        c->fr_in_bytes = 0;
+        CU(cudaMalloc(&c->d_fr_in, in_bytes));
+        c->fr_in_bytes = in_bytes;
+    }
+    return LIINIT_OK;
+}
+
+// argument checks shared by both message types; R = required_cut_num
+int frame_check(Ctx* c, const liinit_frame_params* p, int n, int cap, bool pcl2, int* R) {
+    const int t = p->lidar_type;
+    if (pcl2 ? !(t == LIINIT_LIDAR_VELO || t == LIINIT_LIDAR_OUSTER || t == LIINIT_LIDAR_PANDAR || t == LIINIT_LIDAR_ROBOSENSE) : t != LIINIT_LIDAR_AVIA)
+        return fail(c, LIINIT_ERR_INVALID, "lidar_type does not match the message type");
+    if (p->point_filter_num <= 0 || p->required_frame_num <= 0 || p->required_frame_num > LIINIT_FRAME_MAX_CUT)
+        return fail(c, LIINIT_ERR_INVALID, "point_filter_num must be positive and required_frame_num in [1, LIINIT_FRAME_MAX_CUT]");
+    if (n > c->stage_pts_cap) return fail(c, LIINIT_ERR_CAPACITY, "message exceeds the raw staging capacity");
+    *R = p->scan_count < (pcl2 ? 20 : 5) ? 1 : p->required_frame_num;
+    if (n > 0 && cap < *R) return fail(c, LIINIT_ERR_CAPACITY, "cap is smaller than required_cut_num");
+    return LIINIT_OK;
+}
+
+// flags and decoded points are in place, tsum holds the per-block flag counts: compaction, time sort, cut, gather, table
+int frame_finish(Ctx* c, int n, int R, double S, int* tsum, liinit_subframe* out, int* n_sub) {
+    const int nb = nblk(n, LI_FR_TILE);
+    k_rs_scan<<<1, 1024, 0, c->stream>>>(nb, tsum);
+    k_fr_compact<<<nb, LI_FR_TILE, 0, c->stream>>>(c->d_fr_flag, n, tsum, c->d_fr_dec, nullptr, c->d_fr_keys, c->d_fr_vals, &c->d_fr_tab->V);
+    unsigned *k0 = c->d_fr_keys, *v0 = c->d_fr_vals, *k1 = c->d_rs_keys, *v1 = c->d_rs_vals;
+    const int ntiles = nblk(n, RS_TILE);
+    for (int pass = 0; pass < 4; pass++) {
+        k_rs_hist_dev<<<nblk(ntiles, 4), 128, 0, c->stream>>>(k0, &c->d_fr_tab->V, 8 * pass, ntiles, c->d_rs_hist);
+        k_rs_scan<<<1, 1024, 0, c->stream>>>(256 * ntiles, c->d_rs_hist);
+        k_rs_scatter_dev<<<nblk(ntiles, 4), 128, 0, c->stream>>>(k0, v0, &c->d_fr_tab->V, 8 * pass, ntiles, c->d_rs_hist, k1, v1);
+        unsigned* t = k0; k0 = k1; k1 = t;
+        t = v0; v0 = v1; v1 = t;
+    }
+    const int slot = (int)(c->fr_seq % LIINIT_FRAME_SLOTS);
+    const size_t cap = (size_t)c->stage_pts_cap;
+    k_fr_bounds<<<1, 32, 0, c->stream>>>(v0, c->d_fr_dec, R, S, c->d_fr_tab);
+    k_fr_gather<<<nblk(n, 256), 256, 0, c->stream>>>(v0, c->d_fr_dec, c->d_fr_inten, S, c->d_fr_tab, c->d_fr_slot_pts + slot * cap,
+                                                     c->d_fr_slot_inten + slot * cap);
+    c->launches += 16;
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(c->h_fr_tab, c->d_fr_tab, offsetof(FrameTable, sub) + (size_t)R * sizeof(FrameSub), cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    const FrameTable* T = c->h_fr_tab;
+    if (T->err & 1) return fail(c, LIINIT_ERR_INVALID, "ring >= 128 in the constant-rotation model");
+    *n_sub = T->nsub;
+    if (T->nsub == 0) return LIINIT_OK;
+    c->fr_slot_seq[slot] = c->fr_seq;
+    c->fr_slot_nsub[slot] = T->nsub;
+    for (int k = 0; k < T->nsub; k++) {
+        c->fr_slot_sub[slot][k] = T->sub[k];
+        out[k].handle = c->fr_seq * LIINIT_FRAME_MAX_CUT + k;
+        out[k].t_beg = T->sub[k].lfet / double(1000);
+        out[k].end_ms = T->sub[k].end_ms;
+        out[k].n = T->sub[k].n;
+    }
+    c->fr_seq++;
+    return LIINIT_OK;
+}
+
+// the sub-frame a handle names, or nullptr when its slot has been reused
+const FrameSub* frame_lookup(Ctx* c, long long handle, int* slot) {
+    if (!c->fr_ready || handle < 0) return nullptr;
+    const long long seq = handle / LIINIT_FRAME_MAX_CUT;
+    const int k = (int)(handle % LIINIT_FRAME_MAX_CUT);
+    const int s = (int)(seq % LIINIT_FRAME_SLOTS);
+    if (c->fr_slot_seq[s] != seq || k >= c->fr_slot_nsub[s]) return nullptr;
+    *slot = s;
+    return &c->fr_slot_sub[s][k];
+}
+
 }  // namespace
 
 struct liinit_ctx {
@@ -755,6 +897,7 @@ int liinit_destroy(liinit_ctx* h) {
     if (c->comm) { NcclApi* N = nccl_api(); if (N) N->CommDestroy(c->comm); c->comm = nullptr; }
 #endif
     cudaFree(c->d_partials); cudaFree(c->d_done); cudaFreeHost(c->h_out); cudaFree(c->d_q_d2);
+    frame_free(c);
     if (c->ev0) cudaEventDestroy(c->ev0);
     if (c->ev1) cudaEventDestroy(c->ev1);
     if (c->evm) cudaEventDestroy(c->evm);
@@ -1129,6 +1272,138 @@ int liinit_raw_undistort_imu(liinit_ctx* h, const double* poses, int npose, cons
     k_undistort_imu<<<nblk(c->raw_n, 256), 256, 0, c->stream>>>(c->d_stage_pts, c->raw_n, c->d_poses, npose, S);
     c->launches++;
     CU(cudaGetLastError());
+    return LIINIT_OK;
+}
+
+int liinit_frame_cut_livox(liinit_ctx* h, const void* pts, int stride, int n, const liinit_frame_params* p, liinit_subframe* out, int cap,
+                           int* n_sub) {
+    if (!h || !p || !n_sub || n < 0 || (n > 0 && (!pts || !out))) return LIINIT_ERR_INVALID;
+    Ctx* c = &h->c;
+    CU(cudaSetDevice(c->device));
+    if (stride < 19) return fail(c, LIINIT_ERR_INVALID, "stride_bytes must be at least 19 (CustomPoint)");
+    int R = 1;
+    int r = frame_check(c, p, n, cap, false, &R);
+    if (r) return r;
+    *n_sub = 0;
+    if (n == 0) return LIINIT_OK;
+    r = frame_alloc(c, (size_t)n * stride);
+    if (r) return r;
+    CU(cudaMemcpyAsync(c->d_fr_in, pts, (size_t)n * stride, cudaMemcpyHostToDevice, c->stream));
+    CU(cudaMemsetAsync(c->d_fr_tab, 0, offsetof(FrameTable, sub), c->stream));
+    const int nb = nblk(n, LI_FR_TILE);
+    int* tsum = c->d_fr_tsum;
+    int* tsum2 = c->d_fr_tsum + frame_tiles(c);
+    k_fr_lvx_valid<<<nb, LI_FR_TILE, 0, c->stream>>>(c->d_fr_in, stride, n, p->N_SCANS, c->d_fr_flag, tsum);
+    k_rs_scan<<<1, 1024, 0, c->stream>>>(nb, tsum);
+    k_fr_lvx_keep<<<nb, LI_FR_TILE, 0, c->stream>>>(c->d_fr_in, stride, n, p->N_SCANS, p->point_filter_num, p->blind * p->blind, tsum, c->d_fr_flag,
+                                                    c->d_fr_dec, c->d_fr_inten, tsum2);
+    c->launches += 3;
+    CU(cudaGetLastError());
+    return frame_finish(c, n, R, p->stamp * 1000, tsum2, out, n_sub);
+}
+
+int liinit_frame_cut_pcl2(liinit_ctx* h, const void* data, const liinit_pcl2_layout* lay, int n, const liinit_frame_params* p,
+                          liinit_subframe* out, int cap, int* n_sub) {
+    if (!h || !p || !lay || !n_sub || n < 0 || (n > 0 && (!data || !out))) return LIINIT_ERR_INVALID;
+    Ctx* c = &h->c;
+    CU(cudaSetDevice(c->device));
+    int R = 1;
+    int r = frame_check(c, p, n, cap, true, &R);
+    if (r) return r;
+    const int t = p->lidar_type;
+    const int isz = t == LIINIT_LIDAR_ROBOSENSE ? 1 : 4;
+    const int tsz = (t == LIINIT_LIDAR_PANDAR || t == LIINIT_LIDAR_ROBOSENSE) ? 8 : 4;
+    const int rsz = t == LIINIT_LIDAR_OUSTER ? 1 : 2;
+    const int offs[6] = {lay->off_x, lay->off_y, lay->off_z, lay->off_intensity, lay->off_time, lay->off_ring};
+    const int sizes[6] = {4, 4, 4, isz, tsz, rsz};
+    if (lay->point_step <= 0) return fail(c, LIINIT_ERR_INVALID, "point_step must be positive");
+    for (int f = 0; f < 6; f++)
+        if (offs[f] < -1 || (offs[f] >= 0 && offs[f] + sizes[f] > lay->point_step))
+            return fail(c, LIINIT_ERR_INVALID, "a field lies outside point_step");
+    *n_sub = 0;
+    if (n == 0) return LIINIT_OK;
+    Pcl2Dev L{lay->point_step, lay->off_x, lay->off_y, lay->off_z, lay->off_intensity, lay->off_time, lay->off_ring, t, 0, 0.0};
+    const unsigned char* bytes = static_cast<const unsigned char*>(data);
+    if (t == LIINIT_LIDAR_VELO || t == LIINIT_LIDAR_ROBOSENSE) {
+        // the rotation model runs when the LAST point's time field is not positive (preprocess.cpp:133,246)
+        double last = 0.0;
+        if (lay->off_time >= 0) {
+            const unsigned char* q = bytes + (size_t)(n - 1) * lay->point_step + lay->off_time;
+            if (t == LIINIT_LIDAR_VELO) { float v; memcpy(&v, q, 4); last = v; }
+            else memcpy(&last, q, 8);
+        }
+        L.yaw = !(last > 0);
+    }
+    if (t == LIINIT_LIDAR_PANDAR && lay->off_time >= 0) memcpy(&L.ts0, bytes + lay->off_time, 8);
+    r = frame_alloc(c, (size_t)n * lay->point_step);
+    if (r) return r;
+    CU(cudaMemcpyAsync(c->d_fr_in, data, (size_t)n * lay->point_step, cudaMemcpyHostToDevice, c->stream));
+    CU(cudaMemsetAsync(c->d_fr_tab, 0, offsetof(FrameTable, sub), c->stream));
+    const int nb = nblk(n, LI_FR_TILE);
+    int* tsum = c->d_fr_tsum;
+    k_fr_pcl2_decode<<<nb, LI_FR_TILE, 0, c->stream>>>(c->d_fr_in, n, L, p->N_SCANS, p->point_filter_num, p->blind * p->blind, p->stamp,
+                                                       c->d_fr_flag, c->d_fr_dec, c->d_fr_inten, c->d_fr_aux, tsum, &c->d_fr_tab->err);
+    c->launches++;
+    if (L.yaw) {
+        // survivors of the blind / NaN test, stably sorted by ring (one 8-bit pass: rings >= 255 are clamped, >= 128 is an error)
+        int* ring_first = c->d_fr_ring;
+        int* ring_desc = c->d_fr_ring + 256;
+        int* n_surv = c->d_fr_ring + 512;
+        const int ntiles = nblk(n, RS_TILE);
+        float* base = reinterpret_cast<float*>(c->d_fr_aux);
+        k_rs_scan<<<1, 1024, 0, c->stream>>>(nb, tsum);
+        k_fr_compact<<<nb, LI_FR_TILE, 0, c->stream>>>(c->d_fr_flag, n, tsum, c->d_fr_dec, c->d_fr_aux, c->d_fr_keys, c->d_fr_vals, n_surv);
+        k_rs_hist_dev<<<nblk(ntiles, 4), 128, 0, c->stream>>>(c->d_fr_keys, n_surv, 0, ntiles, c->d_rs_hist);
+        k_rs_scan<<<1, 1024, 0, c->stream>>>(256 * ntiles, c->d_rs_hist);
+        k_rs_scatter_dev<<<nblk(ntiles, 4), 128, 0, c->stream>>>(c->d_fr_keys, c->d_fr_vals, n_surv, 0, ntiles, c->d_rs_hist, c->d_rs_keys,
+                                                                 c->d_rs_vals);
+        k_fr_yaw_first<<<nblk(n, 256), 256, 0, c->stream>>>(c->d_rs_keys, c->d_rs_vals, n_surv, c->d_fr_dec, c->d_fr_yaw, ring_first, ring_desc);
+        k_fr_yaw_base<<<nblk(n, 256), 256, 0, c->stream>>>(c->d_rs_keys, n_surv, c->d_fr_yaw, ring_first, base, ring_desc);
+        k_fr_yaw_final<<<nblk(n, 256), 256, 0, c->stream>>>(c->d_rs_keys, c->d_rs_vals, n_surv, base, ring_first, ring_desc, p->N_SCANS,
+                                                           p->point_filter_num, c->d_fr_dec, c->d_fr_flag, &c->d_fr_tab->err);
+        k_fr_yaw_chain<<<1, 256, 0, c->stream>>>(c->d_rs_keys, c->d_rs_vals, n_surv, base, ring_first, &c->d_fr_tab->err, c->d_fr_dec);
+        k_fr_tile_count<<<nb, LI_FR_TILE, 0, c->stream>>>(c->d_fr_flag, n, tsum);
+        c->launches += 10;
+    }
+    CU(cudaGetLastError());
+    return frame_finish(c, n, R, p->stamp * 1000, tsum, out, n_sub);
+}
+
+int liinit_frame_stage(liinit_ctx* h, long long handle) {
+    if (!h) return LIINIT_ERR_INVALID;
+    Ctx* c = &h->c;
+    CU(cudaSetDevice(c->device));
+    int slot = 0;
+    const FrameSub* s = frame_lookup(c, handle, &slot);
+    if (!s) return fail(c, LIINIT_ERR_INVALID, "unknown sub-frame handle (its message slot has been reused)");
+    CU(cudaMemcpyAsync(c->d_stage_pts, c->d_fr_slot_pts + (size_t)slot * c->stage_pts_cap + (s->lo - 1), (size_t)s->n * sizeof(float4),
+                       cudaMemcpyDeviceToDevice, c->stream));
+    c->raw_n = s->n;
+    return LIINIT_OK;
+}
+
+int liinit_frame_download(liinit_ctx* h, long long handle, float* pts12, int cap, int* n) {
+    if (!h || !n) return LIINIT_ERR_INVALID;
+    Ctx* c = &h->c;
+    CU(cudaSetDevice(c->device));
+    int slot = 0;
+    const FrameSub* s = frame_lookup(c, handle, &slot);
+    if (!s) return fail(c, LIINIT_ERR_INVALID, "unknown sub-frame handle (its message slot has been reused)");
+    *n = s->n;
+    if (!pts12) return LIINIT_OK;
+    if (cap < s->n) return fail(c, LIINIT_ERR_CAPACITY, "cap_points is smaller than the sub-frame");
+    std::vector<float4> P(s->n);
+    std::vector<float> I(s->n);
+    const size_t o = (size_t)slot * c->stage_pts_cap + (s->lo - 1);
+    CU(cudaMemcpyAsync(P.data(), c->d_fr_slot_pts + o, (size_t)s->n * sizeof(float4), cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaMemcpyAsync(I.data(), c->d_fr_slot_inten + o, (size_t)s->n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    for (int i = 0; i < s->n; i++) {
+        float* q = pts12 + 12 * (size_t)i;
+        q[0] = P[i].x; q[1] = P[i].y; q[2] = P[i].z; q[3] = 1.f;   // PointXYZINormal(): data[3] = 1, normals 0
+        q[4] = q[5] = q[6] = q[7] = 0.f;
+        q[8] = I[i]; q[9] = P[i].w; q[10] = q[11] = 0.f;
+    }
     return LIINIT_OK;
 }
 

@@ -5,6 +5,8 @@ the device map -> map_incremental -> LI-Init data accumulation.
 process_raw: the whole loop body on a raw, timed scan, in both modes -- LiDAR-only (constant-velocity propagation, device
 undistortion) and, after the hand-over of LI_Initialization, LIO (IMU propagation, device undistortion from the IMU pose table);
 then the device voxel grid, the update and map_incremental.
+lidar_cbk_livox / lidar_cbk_pcl2 + process_next: the node's LiDAR callbacks with the cut-frame preprocess on the device and
+sync_packages: a driver message is cut into sub-frames that stay on the device until process_next stages one for the loop body.
 
 Host-side mirror used by the replay tool and the end-to-end tests; every step is one call into the native libraries
 (libliinit_host.so: liinit_propagate_cv, liinit_imu_*, liinit_scan_update; libliinit_gpu.so: liinit_raw_* / liinit_scan_upload /
@@ -61,6 +63,15 @@ class ImuBuffer:
             r[0] -= self.time_lag
 
 
+class SubFrame:
+    """A sub-frame held on the device (an entry of liinit_frame_cut_*), as process_raw's scan."""
+
+    def __init__(self, entry):
+        self.handle = int(entry["handle"])
+        self.end_ms = np.float32(entry["end_ms"])
+        self.n = int(entry["n"])
+
+
 class LidarOdometry:
     def __init__(self, gpu: capi.LiInitGpu, filter_size_map: float, max_iteration: int = 4, gyr_cov: float = 0.1, acc_cov: float = 0.1,
                  orig_odom_freq: int = 10, cut_frame_num: int = 1, data_accum_length: float = 300.0, calib: LiCalib | None = None,
@@ -93,6 +104,13 @@ class LidarOdometry:
             self.imu_proc.set_cov(which, v)
         self.lidar_end_time = None
         self.switch_scan = None   # index (frame_num) of the scan that switched to LIO mode
+        # the LiDAR callbacks (laserMapping.cpp:310-381): preprocess/* parameters with the node's defaults (:768,781-786)
+        self.preprocess = dict(lidar_type=1, N_SCANS=16, blind=1.0, point_filter_num=2)
+        self.scan_count = 0
+        self.last_timestamp_lidar = 0.0
+        self.timediff_set = False
+        self.lidar_buffer = deque()   # lidar_buffer + time_buffer: sub-frame entries {handle, t_beg, end_ms, n} of liinit_frame_cut_*
+        self.dropped_subframes = 0
 
     def push_imu(self, omg, acc, t, mean_acc_norm=9.81):
         """imu_cbk in LO mode (:428-430)."""
@@ -140,8 +158,12 @@ class LidarOdometry:
         undistortion from the IMU pose table. The first scan after the hand-over only switches the IMU processor: like Process, it
         neither propagates nor touches the undistorted cloud, so the cloud of the previous scan -- still staged on the device -- is
         downsampled and matched again (the reference keeps feats_undistort, :909-918)."""
-        raw = np.ascontiguousarray(raw_pts12, np.float32)
-        end_ms = float(raw[:, 9].max())                     # points.back().curvature of the time-sorted cloud
+        if isinstance(raw_pts12, SubFrame):
+            raw = raw_pts12
+            end_ms = float(raw.end_ms)
+        else:
+            raw = np.ascontiguousarray(raw_pts12, np.float32)
+            end_ms = float(raw[:, 9].max())                 # points.back().curvature of the time-sorted cloud
         t_end = t_beg + end_ms / 1000.0                     # lidar_end_time (:455-456)
         group = self.imu_buffer.pop(t_end) if imu_group is None else np.asarray(imu_group, float).reshape(-1, 7)
         if not self.imu_en:
@@ -185,6 +207,58 @@ class LidarOdometry:
             self.data_accum_finished = ok
         return self.state
 
+    # ---- the LiDAR callbacks and sync_packages over the device cut ----
+    def _lidar_cbk(self, stamp: float):
+        """The part of livox_pcl_cbk / standard_pcl_cbk before the cut (:312-324)."""
+        self.scan_count += 1
+        if stamp < self.last_timestamp_lidar:           # "lidar loop back, clear buffer"
+            self.lidar_buffer.clear()
+        self.last_timestamp_lidar = stamp
+        ib = self.imu_buffer
+        if ib.rows and abs(ib.last_stamp - stamp) > 1.0 and not self.timediff_set:   # self sync of IMU and LiDAR clocks
+            self.timediff_set = True
+            ib.timediff = ib.last_stamp - stamp
+
+    def _cut_params(self, stamp):
+        return dict(self.preprocess, required_frame_num=self.cut_frame_num, scan_count=self.scan_count, stamp=float(stamp))
+
+    def lidar_cbk_livox(self, records, stamp: float):
+        """livox_pcl_cbk with cut_frame (:310-345): records = the CustomMsg points (capi.LIVOX_POINT / LIVOX_POINT_ALIGNED),
+        stamp = header.stamp [s]. The sub-frames stay on the device; their entries are appended to lidar_buffer."""
+        self._lidar_cbk(stamp)
+        self.lidar_buffer.extend(self.g.frame_cut_livox(records, **self._cut_params(stamp)))
+
+    def lidar_cbk_pcl2(self, data, layout, n: int, stamp: float):
+        """standard_pcl_cbk with cut_frame (:347-381) for Velodyne, Ouster, Pandar and Robosense PointCloud2 messages."""
+        self._lidar_cbk(stamp)
+        self.lidar_buffer.extend(self.g.frame_cut_pcl2(data, layout, n, **self._cut_params(stamp)))
+
+    def process_next(self):
+        """sync_packages (:436-480) and the loop body on the oldest buffered sub-frame: sub-frames of <= 1 point are dropped; the
+        sub-frame waits until an IMU stamp >= its lidar_end_time has arrived. Sub-frames whose message slot the device has reused
+        (LIINIT_FRAME_SLOTS later messages have yielded sub-frames) are dropped and counted in dropped_subframes. Returns the posterior
+        state, or None when nothing is ready."""
+        while self.lidar_buffer:
+            e = self.lidar_buffer[0]
+            if e["n"] <= 1:                                 # "Too few input point cloud!"
+                self.lidar_buffer.popleft()
+            elif self.g.frame_size(e["handle"]) is None:
+                # the device keeps the sub-frames of the last LIINIT_FRAME_SLOTS messages only: when the loop fell that far behind
+                # the callbacks, the older sub-frames are gone and are skipped before any state is touched
+                self.lidar_buffer.popleft()
+                self.dropped_subframes += 1
+            else:
+                break
+        if not self.lidar_buffer or not self.imu_buffer.rows:
+            return None
+        e = self.lidar_buffer[0]
+        t_end = e["t_beg"] + float(np.float32(e["end_ms"])) / 1000.0
+        if not self.imu_buffer.ready(t_end):
+            return None
+        self.lidar_buffer.popleft()
+        group = self.imu_buffer.pop(t_end)
+        return self.process_raw(SubFrame(e), e["t_beg"], group)
+
     def world_cloud(self):
         """The undistorted raw cloud of the last process_raw in the world frame with the current state (publish_frame_world with
         dense_publish_en, pcd_save; laserMapping.cpp:560-603), [n, 3] float32 in upload order."""
@@ -209,12 +283,19 @@ class LidarOdometry:
     def _propagate_imu(self, state, group, t_beg, end_ms):
         return self.imu_proc.propagate(state, group, t_beg, end_ms)
 
+    def _stage(self, raw):
+        """Stage the raw cloud of the scan: an uploaded PointType array, or a sub-frame the device already holds."""
+        if isinstance(raw, SubFrame):
+            self.g.frame_stage(raw.handle)
+        else:
+            self.g.raw_upload(raw, 9)
+
     def _undistort_cv(self, raw, state):
-        self.g.raw_upload(raw, 9)
+        self._stage(raw)
         self.g.raw_undistort_cv(state[27:30], state[0:9], state[24:27])   # omega = bias_g, rot_end / vel_end propagated
 
     def _undistort_imu(self, raw, poses, state):
-        self.g.raw_upload(raw, 9)
+        self._stage(raw)
         if len(poses) >= 2:   # (one pose: the back-propagation loop of the reference runs zero times)
             R, p, RLI, TLI = host.state_pose(state)
             self.g.raw_undistort_imu(poses, R, p, RLI, TLI)
@@ -242,6 +323,8 @@ class LidarOdometry:
         s[27:30] = np.asarray(res["gyro_bias"], float)      # bias_g (:1209)
         s[30:33] = np.asarray(res["acc_bias"], float)       # bias_a (:1210)
         self.imu_en = True
+        if self.preprocess["lidar_type"] != 1:             # spinning sensors continue at two sub-frames per message (:1214-1215)
+            self.cut_frame_num = 2
         # (:1217-1228) the buffered IMU stamps move by the total time lag; the IMU processor switches at its next scan
         self.imu_buffer.shift(float(res["time_lag_1"]) + float(res["time_lag_2"]))
         self.imu_proc.set_mean_acc_norm(self.mean_acc_norm)

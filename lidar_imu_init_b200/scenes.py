@@ -333,3 +333,90 @@ def make_config(name: str, seed: int = 1, imu_en: bool = False, open_air_frac: f
     body = scan_points(scene, gt, N, seed=seed + 1, det_range=det, sigma=sig, open_air_frac=open_air_frac, order=order)
     init = perturb_pose(gt, seed + 2)
     return dict(scene=scene, map_xyz=mp, body_xyz=body, pose_gt=gt, pose_init=init, ds=ds, imu_en=imu_en, name=name)
+
+
+# ---- driver messages for the cut-frame preprocess (liinit_frame_cut_*) -------------------------------------------------------
+def livox_message(scene: Scene, pose_at, stamp: float, N: int, seed: int = 2, dur: float = 0.1, n_scans: int = 6, noise_frac: float = 0.0,
+                  bad_line_frac: float = 0.0, zero_frac: float = 0.0, dup_frac: float = 0.0, tie_frac: float = 0.0, aligned: bool = False,
+                  sigma: float = 0.01) -> np.ndarray:
+    """A Livox CustomMsg of one 1/10 s sweep (10 Hz): N records of capi.LIVOX_POINT (19 bytes; aligned -> the 20-byte ROS struct),
+    offset_time in ns from `stamp`, ascending, built from timed_scan_points. Controllable fractions of records get a noise tag
+    ((tag & 0x30) = 0x20 / 0x30), a line >= n_scans, a zero (no-return) point, the previous record's coordinates (consecutive
+    duplicate) or the previous record's offset_time (dual-return tie)."""
+    from .capi import LIVOX_POINT, LIVOX_POINT_ALIGNED
+    rng = np.random.Generator(np.random.PCG64(seed + 7919))
+    pts = timed_scan_points(scene, pose_at, stamp, dur, N, seed=seed, sigma=sigma)
+    m = np.zeros(N, LIVOX_POINT_ALIGNED if aligned else LIVOX_POINT)
+    off = np.round(pts[:, 9].astype(np.float64) * 1e6).astype(np.uint32)
+    xyz = pts[:, 0:3].copy()
+    line = rng.integers(0, n_scans, N)
+    tag = np.where(rng.uniform(size=N) < 0.5, 0x00, 0x10)
+    u = rng.uniform(size=N)
+    tag = np.where(u < noise_frac, rng.choice([0x20, 0x30], N), tag)
+    u = rng.uniform(size=N)
+    line = np.where(u < bad_line_frac, rng.integers(n_scans, n_scans + 3, N), line)
+    u = rng.uniform(size=N)
+    xyz[u < zero_frac] = 0.0
+    for i in np.nonzero(rng.uniform(size=N) < dup_frac)[0]:
+        if i > 0:
+            xyz[i] = xyz[i - 1]
+    for i in np.nonzero(rng.uniform(size=N) < tie_frac)[0]:
+        if i > 0:
+            off[i] = off[i - 1]
+    m["offset_time"] = off
+    m["x"], m["y"], m["z"] = xyz[:, 0], xyz[:, 1], xyz[:, 2]
+    m["reflectivity"] = rng.integers(0, 256, N)
+    m["tag"] = tag
+    m["line"] = line
+    return m
+
+
+# PointCloud2 point layouts of the drivers (the point structs of the reference's preprocess.h, PCL_ADD_POINT4D padding included)
+PCL2_FIELDS = {
+    2: dict(point_step=32, off_x=0, off_y=4, off_z=8, off_intensity=16, off_time=20, off_ring=24),   # velodyne: time f32, ring u16
+    3: dict(point_step=48, off_x=0, off_y=4, off_z=8, off_intensity=16, off_time=20, off_ring=26),   # ouster: t u32, ring u8
+    5: dict(point_step=48, off_x=0, off_y=4, off_z=8, off_intensity=16, off_time=24, off_ring=32),   # pandar: timestamp f64, ring u16
+    6: dict(point_step=32, off_x=0, off_y=4, off_z=8, off_intensity=16, off_time=24, off_ring=18),   # robosense: intensity u8, ring u16, timestamp f64
+}
+
+
+def spinning_pcl2(lidar_type: int, n_rings: int, n_az: int, stamp: float = 0.0, seed: int = 3, with_time: bool = True, turns: float = 1.0,
+                  nan_frac: float = 0.0, zero_frac: float = 0.0, extra_pad: int = 0, dur: float = 0.1, az0_deg: float = 30.0):
+    """A spinning LiDAR's PointCloud2 (lidar_type 2 Velodyne, 3 Ouster, 5 Pandar, 6 Robosense): n_az firings of n_rings rings, ring-
+    ordered within a firing, the head turning clockwise (yaw decreasing) by `turns` revolutions over `dur` seconds, ranges 2-40 m.
+    with_time = False leaves the time field out of the layout (Velodyne / Robosense then take the constant-rotation model).
+    Returns (data bytes as uint8 array, layout dict, n). extra_pad adds unused bytes to every point."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    lay = dict(PCL2_FIELDS[lidar_type])
+    lay["point_step"] += int(extra_pad)
+    if not with_time:
+        lay["off_time"] = -1
+    n = n_rings * n_az
+    j = np.repeat(np.arange(n_az), n_rings)
+    ring = np.tile(np.arange(n_rings), n_az)
+    t = dur * j / n_az + rng.uniform(0.0, 1e-6, n)                      # seconds from stamp
+    az = np.deg2rad(az0_deg - 360.0 * turns * j / n_az + rng.normal(0.0, 0.02, n))
+    el = np.deg2rad(-15.0 + 30.0 * ring / max(n_rings - 1, 1))
+    r = rng.uniform(2.0, 40.0, n)
+    xyz = np.stack([r * np.cos(el) * np.cos(az), r * np.cos(el) * np.sin(az), r * np.sin(el)], 1).astype(np.float32)
+    xyz[rng.uniform(size=n) < nan_frac] = np.nan
+    xyz[rng.uniform(size=n) < zero_frac] = 0.0
+    buf = np.zeros((n, lay["point_step"]), np.uint8)
+
+    def put(off, arr, dt):
+        if off >= 0:
+            a = np.ascontiguousarray(np.asarray(arr).astype(dt))
+            buf[:, off:off + a.dtype.itemsize] = a.view(np.uint8).reshape(n, a.dtype.itemsize)
+
+    put(lay["off_x"], xyz[:, 0], "<f4")
+    put(lay["off_y"], xyz[:, 1], "<f4")
+    put(lay["off_z"], xyz[:, 2], "<f4")
+    put(lay["off_intensity"], rng.integers(0, 256, n), "u1" if lidar_type == 6 else "<f4")
+    put(lay["off_ring"], ring, "u1" if lidar_type == 3 else "<u2")
+    if lidar_type == 2:
+        put(lay["off_time"], t, "<f4")
+    elif lidar_type == 3:
+        put(lay["off_time"], np.round(t * 1e9), "<u4")
+    else:
+        put(lay["off_time"], stamp + t, "<f8")
+    return buf.reshape(-1), lay, n
