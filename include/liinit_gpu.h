@@ -157,7 +157,7 @@ int liinit_frame_download(liinit_ctx* h, long long handle, float* pts12, int cap
 int liinit_raw_download(liinit_ctx* h, float* xyz, int cap_points, int* n);
 /* The staged (undistorted) raw cloud in the world frame, packed xyz in upload order: pointBodyToWorld (laserMapping.cpp:209-220)
  * with the given state, the same arithmetic as the map update. This is feats_undistort as publish_frame_world publishes it with
- * dense_publish_en (:563) and as pcd_save accumulates it (:594-603); intensities can be joined by index on the host.
+ * dense_publish_en (:563) and as pcd_save accumulates it (:594-603); liinit_cloud_download returns it with its attributes.
  * *n = number of staged points; xyz may be NULL to ask for it. LIINIT_ERR_CAPACITY when cap_points < *n (nothing is written),
  * LIINIT_ERR_INVALID when no raw cloud is staged. */
 int liinit_raw_download_world(liinit_ctx* h, const double rot_end[9], const double pos_end[3], const double R_LI[9], const double T_LI[3],
@@ -192,6 +192,31 @@ int liinit_scan_download_effect(liinit_ctx* h, float* ori_xyz, float* normvec, i
  * near_xyz [n*5*3] + near_cnt [n] (Nearest_Points), selected [n] (point_selected_surf), normvec [n*4]. */
 int liinit_scan_download_state(liinit_ctx* h, float* world_xyz, float* near_xyz, int* near_cnt, unsigned char* selected,
                                float* normvec);
+/* ---- published clouds (publish_frame_world, publish_frame_body, publish_effect_world and pcd_save, laserMapping.cpp:561-636) ----
+ * One cloud as 48-byte pcl::PointXYZINormal records, 12 floats {x, y, z, 1, normal_x, normal_y, normal_z, 0, intensity, curvature, 0, 0}:
+ * the data of the sensor_msgs/PointCloud2 that pcl::toROSMsg makes of a PointCloudXYZI (point_step 48; FLOAT32 fields x@0, y@4, z@8,
+ * normal_x@16, normal_y@20, normal_z@24, intensity@32, curvature@36; the padding floats are 0). The world-frame clouds are
+ * pointBodyToWorld (:209-220) with the given state into fresh points: xyz transformed, normals and intensity copied, curvature 0.
+ *   REGISTERED       the staged, undistorted raw cloud (feats_undistort) in staging order; xyz bit-equal to liinit_raw_download_world.
+ *                    Normals and intensity: floats 4-6 and 8 of a liinit_raw_upload(pts, >= 12, 9, n) point, the message intensity of a
+ *                    liinit_frame_stage sub-frame (normals 0), zeros for any other upload.
+ *   REGISTERED_DOWN  the resident scan (feats_down_body) made by liinit_raw_downsample: normals and intensity are leaf means, as PCL's
+ *                    VoxelGrid with downsample_all_data_ computes them (input-order sums, divided by the count like the xyz); zeros
+ *                    for a scan uploaded as xyz.
+ *   BODY             the staged, undistorted raw cloud as it is: curvature = its time offset [ms]. The pose arguments may be NULL.
+ *   EFFECT           laserCloudOri: the resident-scan points the last ICP pass selected, in index order (effect_feat_num of them, the
+ *                    count liinit_scan_download_effect returns), intensity sqrt(1000) as the Jacobian loop leaves it (:1050-1051).
+ *                    With a communicator attached this is collective (the flags of every rank's slot are all-gathered first); every rank
+ *                    receives the whole frame's cloud.
+ * rec12 may be NULL to ask for *n. LIINIT_ERR_CAPACITY when cap_points < *n (nothing written). LIINIT_ERR_INVALID for an unknown
+ * `which`, no staged raw cloud (REGISTERED, BODY), no resident scan (REGISTERED_DOWN), no ICP pass on the resident scan (EFFECT).
+ * No call changes any state: the update and map_incremental give the same results with or without these calls in between. */
+#define LIINIT_CLOUD_REGISTERED 1       /* feats_undistort -> world  (publish_frame_world with dense_pub_en; pcd_save) */
+#define LIINIT_CLOUD_REGISTERED_DOWN 2  /* feats_down_body -> world  (publish_frame_world without dense_pub_en) */
+#define LIINIT_CLOUD_BODY 3             /* feats_undistort as it is  (publish_frame_body) */
+#define LIINIT_CLOUD_EFFECT 4           /* laserCloudOri -> world    (publish_effect_world) */
+int liinit_cloud_download(liinit_ctx* h, int which, const double rot_end[9], const double pos_end[3], const double R_LI[9],
+                          const double T_LI[3], float* rec12, int cap_points, int* n);
 /* map_incremental (laserMapping.cpp:516-559) with the final state; uses the neighbour lists retained on the
  * device by the last search pass. ds = the node's double filter_size_map_min. n_add / n_no_downsample:
  * sizes of PointToAdd / PointNoNeedDownsample. */

@@ -42,6 +42,16 @@ class SubFrame(C.Structure):   # liinit_subframe
 
 
 FRAME_MAX_CUT = 256   # LIINIT_FRAME_MAX_CUT
+# liinit_cloud_download: the node's published clouds
+CLOUD_REGISTERED = 1        # feats_undistort -> world (publish_frame_world with dense_pub_en; pcd_save)
+CLOUD_REGISTERED_DOWN = 2   # feats_down_body -> world (publish_frame_world without dense_pub_en)
+CLOUD_BODY = 3              # feats_undistort as it is (publish_frame_body)
+CLOUD_EFFECT = 4            # laserCloudOri -> world (publish_effect_world)
+# the sensor_msgs/PointCloud2 of pcl::toROSMsg(PointCloudXYZI) whose data the [n, 12] float32 records are: (name, offset, datatype,
+# count); datatype 7 = FLOAT32
+POINTCLOUD2_POINT_STEP = 48
+POINTCLOUD2_FIELDS = (("x", 0, 7, 1), ("y", 4, 7, 1), ("z", 8, 7, 1), ("normal_x", 16, 7, 1), ("normal_y", 20, 7, 1), ("normal_z", 24, 7, 1),
+                      ("intensity", 32, 7, 1), ("curvature", 36, 7, 1))
 # Livox CustomPoint: 19 bytes on the wire, 20 as the ROS struct (align=True)
 LIVOX_POINT = np.dtype([("offset_time", "<u4"), ("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("reflectivity", "u1"), ("tag", "u1"), ("line", "u1")])
 LIVOX_POINT_ALIGNED = np.dtype(LIVOX_POINT, align=True)
@@ -56,7 +66,7 @@ SYMBOLS = [
     "liinit_raw_download", "liinit_raw_download_world", "liinit_raw_downsample",
     "liinit_frame_cut_livox", "liinit_frame_cut_pcl2", "liinit_frame_stage", "liinit_frame_download",
     "liinit_icp_iterate", "liinit_icp_iterate_device", "liinit_scan_download_effect", "liinit_scan_download_state",
-    "liinit_map_incremental", "liinit_last_pass_timing", "liinit_last_pass_kernel_times", "liinit_launch_count", "liinit_map_stats", "liinit_knn_index",
+    "liinit_cloud_download", "liinit_map_incremental", "liinit_last_pass_timing", "liinit_last_pass_kernel_times", "liinit_launch_count", "liinit_map_stats", "liinit_knn_index",
     "liinit_comm_unique_id", "liinit_comm_init", "liinit_comm_info", "liinit_comm_last_local", "liinit_comm_mode", "liinit_debug_esti_plane", "liinit_set_reseed",
 ]
 
@@ -109,6 +119,7 @@ def load():
     L.liinit_icp_iterate_device.argtypes = [vp, _f64, _f64, _f64, _f64, C.c_int, C.c_int, vp]
     L.liinit_scan_download_effect.argtypes = [vp, vp, vp, C.c_int, C.POINTER(C.c_int)]
     L.liinit_scan_download_state.argtypes = [vp, vp, vp, vp, vp, vp]
+    L.liinit_cloud_download.argtypes = [vp, C.c_int, vp, vp, vp, vp, vp, C.c_int, C.POINTER(C.c_int)]
     L.liinit_map_incremental.argtypes = [vp, _f64, _f64, _f64, _f64, C.c_double, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
     L.liinit_last_pass_timing.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(C.c_int)]
     L.liinit_last_pass_kernel_times.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(C.c_float)]
@@ -376,6 +387,20 @@ class LiInitGpu:
         m = C.c_int(0)
         self._ck(self.L.liinit_scan_download_effect(self.h, _ptr(ori), _ptr(nv), n, C.byref(m)))
         return ori[:m.value], nv[:m.value]
+
+    def cloud(self, which: int, rot_end=None, pos_end=None, R_LI=None, T_LI=None):
+        """One of the node's published clouds (CLOUD_*) as [n, 12] float32 pcl::PointXYZINormal records (the PointCloud2 data of
+        POINTCLOUD2_FIELDS). The world-frame clouds need the pose (the posterior the node publishes with); CLOUD_BODY ignores it."""
+        pose = [None] * 4
+        if rot_end is not None:
+            pose = [np.ascontiguousarray(rot_end, np.float64).reshape(9), np.ascontiguousarray(pos_end, np.float64).reshape(3),
+                    np.ascontiguousarray(R_LI, np.float64).reshape(9), np.ascontiguousarray(T_LI, np.float64).reshape(3)]
+        args = [_ptr(a) for a in pose]
+        n = C.c_int(0)
+        self._ck(self.L.liinit_cloud_download(self.h, int(which), *args, None, 0, C.byref(n)))
+        out = np.zeros((n.value, 12), np.float32)
+        self._ck(self.L.liinit_cloud_download(self.h, int(which), *args, _ptr(out), n.value, C.byref(n)))
+        return out
 
     def map_incremental(self, rot_end, pos_end, R_LI, T_LI, ds: float, flg_EKF_inited: bool = True):
         na, nn = C.c_int(0), C.c_int(0)

@@ -26,6 +26,7 @@
 #include "voxelgrid_kernels.cuh"
 #include "undistort_kernels.cuh"
 #include "preprocess_kernels.cuh"
+#include "output_kernels.cuh"
 
 #ifndef LI_CELLS_MINB
 #define LI_CELLS_MINB 6
@@ -103,13 +104,15 @@ struct Ctx {
     float* d_stage_raw = nullptr;   // strided host layout
     size_t stage_raw_floats = 0;
     float4* d_stage_pts = nullptr;  // repacked batch
+    float4* d_stage_attr = nullptr; // attribute channel of the staged raw cloud: {normal_x, normal_y, normal_z, intensity} per point
+    bool stage_attr = false;        // ... filled by the last raw upload / frame stage (otherwise it reads as zeros)
     int stage_pts_cap = 0;
     int* d_slot_of = nullptr;
     int* d_vslot_of = nullptr;
     int* d_flag = nullptr;
     int* d_ins = nullptr;
     int* d_vg_imin = nullptr;      // voxel-grid: first point index per leaf
-    int* d_vg_block = nullptr;     // (unused scratch)
+    int* d_vg_block = nullptr;     // per-block counts of the effect-cloud compaction (liinit_cloud_download)
     unsigned* d_rs_keys = nullptr;  // radix sort ping-pong buffers + histogram
     unsigned* d_rs_vals = nullptr;
     int* d_rs_hist = nullptr;
@@ -143,6 +146,8 @@ struct Ctx {
     // scan
     ScanDev S{};
     float4* d_body = nullptr;
+    float4* d_body_attr = nullptr;  // leaf means of the staged attribute channel for a resident scan made by liinit_raw_downsample ...
+    bool body_attr = false;         // ... (an uploaded, xyz-only scan has none: zeros)
     float4* d_world = nullptr;
     int* d_near_ids = nullptr;
     float4* d_near_xyz = nullptr;
@@ -818,6 +823,7 @@ int liinit_create(const liinit_config* cfg, liinit_ctx** out) {
     c->stage_raw_floats = (size_t)batch * 12;
     CUC(cudaMalloc(&c->d_stage_raw, c->stage_raw_floats * 4));
     CUC(cudaMalloc(&c->d_stage_pts, (size_t)batch * sizeof(float4)));
+    CUC(cudaMalloc(&c->d_stage_attr, (size_t)batch * sizeof(float4)));
     CUC(cudaMalloc(&c->d_slot_of, (size_t)batch * sizeof(int)));
     CUC(cudaMalloc(&c->d_vslot_of, (size_t)batch * sizeof(int)));
     CUC(cudaMalloc(&c->d_flag, (size_t)batch * sizeof(int)));
@@ -846,6 +852,7 @@ int liinit_create(const liinit_config* cfg, liinit_ctx** out) {
     CUC(cudaMalloc(&c->d_acc, 160 * sizeof(double)));
     CUC(cudaMalloc(&c->d_red, 160 * sizeof(double)));
     CUC(cudaMalloc(&c->d_body, (size_t)ns * sizeof(float4)));
+    CUC(cudaMalloc(&c->d_body_attr, (size_t)ns * sizeof(float4)));
     CUC(cudaMalloc(&c->d_world, (size_t)ns * sizeof(float4)));
     CUC(cudaMalloc(&c->d_near_ids, (size_t)batch * 5 * sizeof(int)));
     CUC(cudaMalloc(&c->d_near_xyz, (size_t)ns * 5 * sizeof(float4)));
@@ -887,6 +894,7 @@ int liinit_destroy(liinit_ctx* h) {
     cudaFree(c->M.ent); cudaFree(c->M.brick_slots); cudaFree(c->M.aux); cudaFree(c->M.pool); cudaFree(c->M.pool_top); cudaFree(c->M.touched_list); cudaFree(c->M.cocc); cudaFree(c->M.cdir); cudaFree(c->M.sb_keys); cudaFree(c->M.sb_occ); cudaFree(c->d_ticket);
     cudaFree(c->d_counters); cudaFreeHost(c->h_counters); cudaFreeHost(c->h_pool_top); cudaFree(c->d_stage_raw); cudaFree(c->d_stage_pts);
     cudaFree(c->d_slot_of); cudaFree(c->d_vslot_of); cudaFree(c->d_flag); cudaFree(c->d_ins); cudaFree(c->V.keys); cudaFree(c->V.head); cudaFree(c->V.coupled); cudaFree(c->V.sum); cudaFree(c->V.clist); cudaFree(c->d_vg_imin); cudaFree(c->d_vg_block); cudaFree(c->d_vg_misc); cudaFree(c->d_rs_keys); cudaFree(c->d_rs_vals); cudaFree(c->d_rs_hist); cudaFree(c->d_vg_params); cudaFree(c->d_tmin_idx); cudaFree(c->d_poses);
+    cudaFree(c->d_stage_attr); cudaFree(c->d_body_attr);
     cudaFree(c->d_body); cudaFree(c->d_world); cudaFree(c->d_near_ids); cudaFree(c->d_near_xyz); cudaFree(c->d_selected); cudaFree(c->d_normvec);
     cudaFree(c->d_acc); cudaFree(c->d_red);
 #ifndef LI_SIMT_EMUL
@@ -1182,6 +1190,7 @@ int liinit_scan_upload(liinit_ctx* h, const float* body, int stride, int n) {
     if (n > c->cfg.max_scan_points) return fail(c, LIINIT_ERR_CAPACITY, "n exceeds max_scan_points");
     c->attached = nullptr;
     c->attached_slot_done = false;
+    c->body_attr = false;
     if (stride == 4) {
         CU(cudaMemcpyAsync(c->d_body, body, (size_t)n * 16, cudaMemcpyHostToDevice, c->stream));
     } else if (stride == 3 || stride == 12) {
@@ -1213,6 +1222,7 @@ int liinit_scan_attach_host(liinit_ctx* h, const float* pinned_body, int stride,
     c->attached = (const float*)at.devicePointer;
     c->attached_stride = stride;
     c->attached_slot_done = false;
+    c->body_attr = false;
     set_scan(c, n);   // (N > 1: the search kernel reads this rank's slot in place; the rest is copied when map_incremental / a download needs it)
     return LIINIT_OK;
 }
@@ -1224,7 +1234,9 @@ int liinit_raw_upload(liinit_ctx* h, const float* pts, int stride, int time_inde
     if (stride < 3 || time_index >= stride || (time_index >= 0 && time_index < 3)) return fail(c, LIINIT_ERR_INVALID, "bad stride / time_index");
     if (n > c->stage_pts_cap || (size_t)n * stride > c->stage_raw_floats) return fail(c, LIINIT_ERR_CAPACITY, "raw cloud exceeds staging capacity");
     CU(cudaMemcpyAsync(c->d_stage_raw, pts, (size_t)n * stride * 4, cudaMemcpyHostToDevice, c->stream));
-    k_repack_t<<<nblk(n, 256), 256, 0, c->stream>>>(c->d_stage_raw, stride, time_index, n, c->d_stage_pts);
+    // the PointType layout (the time in curvature) brings its normals and intensity along; any other layout has none
+    c->stage_attr = stride >= 12 && time_index == 9;
+    k_repack_t<<<nblk(n, 256), 256, 0, c->stream>>>(c->d_stage_raw, stride, time_index, n, c->d_stage_pts, c->stage_attr ? c->d_stage_attr : nullptr);
     c->launches++;
     c->raw_n = n;
     CU(cudaGetLastError());
@@ -1376,8 +1388,12 @@ int liinit_frame_stage(liinit_ctx* h, long long handle) {
     int slot = 0;
     const FrameSub* s = frame_lookup(c, handle, &slot);
     if (!s) return fail(c, LIINIT_ERR_INVALID, "unknown sub-frame handle (its message slot has been reused)");
-    CU(cudaMemcpyAsync(c->d_stage_pts, c->d_fr_slot_pts + (size_t)slot * c->stage_pts_cap + (s->lo - 1), (size_t)s->n * sizeof(float4),
-                       cudaMemcpyDeviceToDevice, c->stream));
+    const size_t o = (size_t)slot * c->stage_pts_cap + (s->lo - 1);
+    CU(cudaMemcpyAsync(c->d_stage_pts, c->d_fr_slot_pts + o, (size_t)s->n * sizeof(float4), cudaMemcpyDeviceToDevice, c->stream));
+    k_attr_from_inten<<<nblk(s->n, 256), 256, 0, c->stream>>>(c->d_fr_slot_inten + o, s->n, c->d_stage_attr);
+    c->launches++;
+    CU(cudaGetLastError());
+    c->stage_attr = true;
     c->raw_n = s->n;
     return LIINIT_OK;
 }
@@ -1479,7 +1495,8 @@ int liinit_raw_downsample(liinit_ctx* h, float leaf_size, int* n_down) {
     }
     (void)nb;
     k_vg_centroid_sorted<<<nblk(n, 256), 256, 0, c->stream>>>(c->d_stage_pts, v0, c->d_vg_misc + 6, c->d_slot_of, V, c->d_vslot_of, c->d_body,
-                                                               c->cfg.max_scan_points, c->d_vg_misc + 7);
+                                                               c->cfg.max_scan_points, c->d_vg_misc + 7, c->stage_attr ? c->d_stage_attr : nullptr,
+                                                               c->d_body_attr);
     c->launches += 12;
     c->launches += 7;
     CU(cudaGetLastError());
@@ -1495,6 +1512,7 @@ int liinit_raw_downsample(liinit_ctx* h, float leaf_size, int* n_down) {
     if (m <= 0) return fail(c, LIINIT_ERR_INVALID, "voxel grid: no output points");
     set_scan(c, m);
     c->attached = nullptr;
+    c->body_attr = c->stage_attr;
     if (n_down) *n_down = m;
     return LIINIT_OK;
 }
@@ -1620,6 +1638,60 @@ int liinit_scan_download_effect(liinit_ctx* h, float* ori_xyz, float* normvec, i
         k++;
     }
     *m = k;
+    return LIINIT_OK;
+}
+
+int liinit_cloud_download(liinit_ctx* h, int which, const double* R, const double* p, const double* RLI, const double* TLI, float* rec12,
+                          int cap, int* n) {
+    if (!h || !n) return LIINIT_ERR_INVALID;
+    Ctx* c = &h->c;
+    CU(cudaSetDevice(c->device));
+    if (which < LIINIT_CLOUD_REGISTERED || which > LIINIT_CLOUD_EFFECT) return fail(c, LIINIT_ERR_INVALID, "unknown cloud");
+    if (which != LIINIT_CLOUD_BODY && (!R || !p || !RLI || !TLI)) return fail(c, LIINIT_ERR_INVALID, "a world-frame cloud needs the pose");
+    const bool raw = which == LIINIT_CLOUD_REGISTERED || which == LIINIT_CLOUD_BODY;
+    if (raw && c->raw_n <= 0) return fail(c, LIINIT_ERR_INVALID, "no raw cloud staged (liinit_raw_upload / liinit_frame_stage)");
+    if (!raw && c->scan_n <= 0) return fail(c, LIINIT_ERR_INVALID, "no scan resident");
+    if (which == LIINIT_CLOUD_EFFECT && !c->have_neighbors) return fail(c, LIINIT_ERR_INVALID, "no ICP pass on the resident scan yet");
+    PoseD P;
+    if (which != LIINIT_CLOUD_BODY) fill_pose(P, R, p, RLI, TLI);
+    // the records are built in the strided staging buffer (12 floats per point of the staging capacity), free once a cloud is repacked
+    float* out = c->d_stage_raw;
+    const float4* battr = c->body_attr ? c->d_body_attr : nullptr;
+    int m = 0;
+    if (raw) {
+        m = c->raw_n;
+    } else if (which == LIINIT_CLOUD_REGISTERED_DOWN) {
+        m = c->scan_n;
+    } else {
+        // laserCloudOri: the points the last pass selected, over the whole frame (N > 1: after the all-gather of the flags)
+        int r = init_scan_state(c);
+        if (r) return r;
+        r = gather_scan_state(c);
+        if (r) return r;
+        const int nb = nblk(c->scan_n, LI_FR_TILE);
+        k_eff_count<<<nb, LI_FR_TILE, 0, c->stream>>>(c->d_selected, c->scan_n, c->d_vg_block);
+        k_rs_scan<<<1, 1024, 0, c->stream>>>(nb + 1, c->d_vg_block);
+        c->launches += 2;
+        CU(cudaGetLastError());
+        CU(cudaMemcpyAsync(&m, c->d_vg_block + nb, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+        CU(cudaStreamSynchronize(c->stream));
+    }
+    *n = m;
+    if (!rec12) return LIINIT_OK;
+    if (cap < m) return fail(c, LIINIT_ERR_CAPACITY, "cap_points is smaller than the cloud");
+    if (m == 0) return LIINIT_OK;
+    if (!raw) materialize_scan(c);   // (an attached host scan: the whole frame into d_body)
+    const float4* sattr = c->stage_attr ? c->d_stage_attr : nullptr;
+    switch (which) {
+        case LIINIT_CLOUD_REGISTERED: k_cloud_world<<<nblk(m, 256), 256, 0, c->stream>>>(c->d_stage_pts, sattr, m, P, out); break;
+        case LIINIT_CLOUD_BODY: k_cloud_body<<<nblk(m, 256), 256, 0, c->stream>>>(c->d_stage_pts, sattr, m, out); break;
+        case LIINIT_CLOUD_REGISTERED_DOWN: k_cloud_world<<<nblk(m, 256), 256, 0, c->stream>>>(c->d_body, battr, m, P, out); break;
+        default: k_eff_emit<<<nblk(c->scan_n, LI_FR_TILE), LI_FR_TILE, 0, c->stream>>>(c->d_selected, c->scan_n, c->d_vg_block, c->d_body, battr, P, out); break;
+    }
+    c->launches++;
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(rec12, out, (size_t)m * 12 * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
     return LIINIT_OK;
 }
 

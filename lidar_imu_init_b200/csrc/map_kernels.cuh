@@ -18,12 +18,14 @@ __global__ void k_repack(const float* __restrict__ src, int stride, int n, float
     dst[i] = make_float4(s[0], s[1], s[2], 0.f);
 }
 
-// same, keeping one more float (a per-point time stamp, e.g. PointType.curvature) in w
-__global__ void k_repack_t(const float* __restrict__ src, int stride, int tidx, int n, float4* __restrict__ dst) {
+// same, keeping one more float (a per-point time stamp, e.g. PointType.curvature) in w; attr (optional, PointType layout only):
+// {normal_x, normal_y, normal_z, intensity} = floats 4-6 and 8
+__global__ void k_repack_t(const float* __restrict__ src, int stride, int tidx, int n, float4* __restrict__ dst, float4* __restrict__ attr) {
     int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const float* s = src + (size_t)i * stride;
     dst[i] = make_float4(s[0], s[1], s[2], tidx >= 0 ? s[tidx] : 0.f);
+    if (attr) attr[i] = make_float4(s[4], s[5], s[6], s[8]);
 }
 
 __global__ void k_map_clear(uint4* ent, uint4* aux, unsigned slots) {

@@ -131,10 +131,12 @@ __global__ void k_vg_collect(VoxTmp V, const int* __restrict__ imin, unsigned* _
     vals[pos] = (unsigned)imin[i];
 }
 
-// one thread per leaf, leaves in ascending leaf index (PCL's output order): sum the leaf's points in input order
+// one thread per leaf, leaves in ascending leaf index (PCL's output order): sum the leaf's points in input order. attr (optional):
+// the attribute channel of the staged points {normal_x, normal_y, normal_z, intensity}, averaged the same way into out_attr
+// (VoxelGrid with downsample_all_data_, the default: every field is a leaf mean; the curvature mean is never published)
 __global__ void k_vg_centroid_sorted(const float4* __restrict__ pts, const unsigned* __restrict__ reps, const int* __restrict__ count,
                                      const int* __restrict__ slot_of, VoxTmp V, int* __restrict__ next_of, float4* __restrict__ out,
-                                     int out_cap, int* __restrict__ err) {
+                                     int out_cap, int* __restrict__ err, const float4* __restrict__ attr, float4* __restrict__ out_attr) {
     int pos = blockIdx.x * blockDim.x + threadIdx.x;
     if (pos >= *count) return;
     if (pos >= out_cap) {
@@ -145,6 +147,7 @@ __global__ void k_vg_centroid_sorted(const float4* __restrict__ pts, const unsig
     // stores; long lists (near-sensor leaves of a dense raw scan): sort the links once (merge sort), then one walk
     int head = V.head[slot_of[reps[pos]]];
     float sx = 0.f, sy = 0.f, sz = 0.f;
+    float ax = 0.f, ay = 0.f, az = 0.f, aw = 0.f;
     int cnt = 0;
     if (li_list_longer_than(head, next_of, LI_LIST_SELECT_MAX)) {
         head = li_list_sort_ascending(head, next_of);
@@ -153,6 +156,10 @@ __global__ void k_vg_centroid_sorted(const float4* __restrict__ pts, const unsig
             sx = __fadd_rn(sx, p.x);
             sy = __fadd_rn(sy, p.y);
             sz = __fadd_rn(sz, p.z);
+            if (attr) {
+                const float4 a = attr[cur];
+                ax = __fadd_rn(ax, a.x); ay = __fadd_rn(ay, a.y); az = __fadd_rn(az, a.z); aw = __fadd_rn(aw, a.w);
+            }
             cnt++;
         }
     } else {
@@ -167,9 +174,14 @@ __global__ void k_vg_centroid_sorted(const float4* __restrict__ pts, const unsig
             sx = __fadd_rn(sx, p.x);
             sy = __fadd_rn(sy, p.y);
             sz = __fadd_rn(sz, p.z);
+            if (attr) {
+                const float4 a = attr[cur];
+                ax = __fadd_rn(ax, a.x); ay = __fadd_rn(ay, a.y); az = __fadd_rn(az, a.z); aw = __fadd_rn(aw, a.w);
+            }
             cnt++;
         }
     }
     float c = (float)cnt;
     out[pos] = make_float4(__fdiv_rn(sx, c), __fdiv_rn(sy, c), __fdiv_rn(sz, c), 0.f);
+    if (attr) out_attr[pos] = make_float4(__fdiv_rn(ax, c), __fdiv_rn(ay, c), __fdiv_rn(az, c), __fdiv_rn(aw, c));
 }

@@ -7,6 +7,8 @@ undistortion) and, after the hand-over of LI_Initialization, LIO (IMU propagatio
 then the device voxel grid, the update and map_incremental.
 lidar_cbk_livox / lidar_cbk_pcl2 + process_next: the node's LiDAR callbacks with the cut-frame preprocess on the device and
 sync_packages: a driver message is cut into sub-frames that stay on the device until process_next stages one for the loop body.
+publish= (off by default): the node's published clouds after every update of process_raw -- /cloud_registered, /cloud_registered_body,
+/cloud_effected as PointCloud2-ready records built on the device -- and pcd_save's PCD files.
 
 Host-side mirror used by the replay tool and the end-to-end tests; every step is one call into the native libraries
 (libliinit_host.so: liinit_propagate_cv, liinit_imu_*, liinit_scan_update; libliinit_gpu.so: liinit_raw_* / liinit_scan_upload /
@@ -14,12 +16,26 @@ liinit_map_*; libliinit_calib.so: li_calib_*). Nothing is computed in Python.
 """
 from __future__ import annotations
 
+import os
 from collections import deque
+from dataclasses import dataclass
 
 import numpy as np
 
-from . import capi, host
+from . import capi, host, pcd
 from .calib import LiCalib
+
+
+@dataclass
+class Publish:
+    """The node's publish/* and pcd_save/* parameters with its defaults (laserMapping.cpp:794-799); set them from the YAML.
+    pcd_dir is where pcd_save writes (the node's root_dir + "/PCD")."""
+    scan_pub_en: bool = True        # publish/scan_publish_en
+    dense_pub_en: bool = True       # publish/dense_publish_en
+    scan_body_pub_en: bool = True   # publish/scan_bodyframe_pub_en
+    pcd_save_en: bool = False       # pcd_save/pcd_save_en
+    interval: int = -1              # pcd_save/interval
+    pcd_dir: str = "PCD"
 
 
 class ImuBuffer:
@@ -76,7 +92,7 @@ class LidarOdometry:
     def __init__(self, gpu: capi.LiInitGpu, filter_size_map: float, max_iteration: int = 4, gyr_cov: float = 0.1, acc_cov: float = 0.1,
                  orig_odom_freq: int = 10, cut_frame_num: int = 1, data_accum_length: float = 300.0, calib: LiCalib | None = None,
                  filter_size_surf: float | None = None, rot_LI_cov: float = 0.00005, trans_LI_cov: float = 0.0005, b_gyr_cov: float = 0.0001,
-                 b_acc_cov: float = 0.0001, mean_acc_norm: float = 9.81):
+                 b_acc_cov: float = 0.0001, mean_acc_norm: float = 9.81, publish: Publish | dict | None = None):
         self.g = gpu
         self.ds = float(filter_size_map)
         self.max_iteration = int(max_iteration)            # "max_iteration", laserMapping.cpp:767
@@ -111,6 +127,13 @@ class LidarOdometry:
         self.timediff_set = False
         self.lidar_buffer = deque()   # lidar_buffer + time_buffer: sub-frame entries {handle, t_beg, end_ms, n} of liinit_frame_cut_*
         self.dropped_subframes = 0
+        # the published clouds of the last process_raw: {"registered", "body", "effect"} -> [n, 12] float32 records
+        self.publish = Publish(**publish) if isinstance(publish, dict) else publish
+        self.published = {}
+        self.pcd_wait = []            # pcl_wait_save, as the REGISTERED records of the scans since the last file
+        self.scan_wait_num = 0
+        self.pcd_index = 0
+        self.pcd_files = []
 
     def push_imu(self, omg, acc, t, mean_acc_norm=9.81):
         """imu_cbk in LO mode (:428-430)."""
@@ -166,6 +189,7 @@ class LidarOdometry:
             end_ms = float(raw[:, 9].max())                 # points.back().curvature of the time-sorted cloud
         t_end = t_beg + end_ms / 1000.0                     # lidar_end_time (:455-456)
         group = self.imu_buffer.pop(t_end) if imu_group is None else np.asarray(imu_group, float).reshape(-1, 7)
+        self.published = {}
         if not self.imu_en:
             # Forward_propagation_without_imu (IMU_Processing.hpp:204-267)
             if self.first_prop:
@@ -199,6 +223,8 @@ class LidarOdometry:
         if not self.imu_en and not self.data_accum_start and np.linalg.norm(p) > 0.05:   # :1145-1149
             self.data_accum_start = True
             self.move_start_time = t_end
+        if self.publish is not None:                        # :1152-1156
+            self._publish(R, p, RLI, TLI)
         self.frame_num += 1                                 # :1160
         if not self.imu_en and not self.data_accum_finished and self.data_accum_start:   # :1190-1196
             bias_g, vel = self.state[27:30], self.state[24:27]
@@ -258,6 +284,50 @@ class LidarOdometry:
         self.lidar_buffer.popleft()
         group = self.imu_buffer.pop(t_end)
         return self.process_raw(SubFrame(e), e["t_beg"], group)
+
+    def _publish(self, R, p, RLI, TLI):
+        """The "Publish points" block of the loop (:1152-1156) with the posterior: publish_frame_world (:561-614) when scan_pub_en or
+        pcd_save_en, publish_frame_body (:616-623) when scan_pub_en and scan_body_pub_en, publish_effect_world (:625-636) always.
+        The records land in self.published; pcd_save accumulates the REGISTERED records on the host."""
+        c = self.publish
+        out = {}
+        reg = None
+        if c.scan_pub_en:
+            which = capi.CLOUD_REGISTERED if c.dense_pub_en else capi.CLOUD_REGISTERED_DOWN
+            out["registered"] = self.g.cloud(which, R, p, RLI, TLI)
+            if c.dense_pub_en:
+                reg = out["registered"]
+        if c.pcd_save_en:
+            self._pcd_save(reg if reg is not None else self.g.cloud(capi.CLOUD_REGISTERED, R, p, RLI, TLI))
+        if c.scan_pub_en and c.scan_body_pub_en:
+            out["body"] = self.g.cloud(capi.CLOUD_BODY)
+        out["effect"] = self.g.cloud(capi.CLOUD_EFFECT, R, p, RLI, TLI)
+        self.published = out
+
+    def _pcd_save(self, reg):
+        """pcd_save (:594-613): feats_undistort in the world frame is appended to pcl_wait_save; with interval > 0 every interval-th
+        scan writes PCD<k>.pcd and starts over."""
+        self.pcd_wait.append(reg)
+        self.scan_wait_num += 1
+        if sum(len(a) for a in self.pcd_wait) > 0 and self.publish.interval > 0 and self.scan_wait_num >= self.publish.interval:
+            self.pcd_index += 1
+            self._pcd_write(f"PCD{self.pcd_index}.pcd")
+            self.pcd_wait = []
+            self.scan_wait_num = 0
+
+    def _pcd_write(self, name):
+        os.makedirs(self.publish.pcd_dir, exist_ok=True)
+        path = os.path.join(self.publish.pcd_dir, name)
+        pcd.write_binary(path, np.concatenate(self.pcd_wait) if self.pcd_wait else np.zeros((0, 12), np.float32))
+        self.pcd_files.append(path)
+
+    def close(self):
+        """The node's shutdown (SigHandle, :183-187): with pcd_save_en and interval < 0 everything accumulated goes to PCD_all.pcd
+        (nothing is written when no point has been accumulated: PCL refuses an empty cloud)."""
+        c = self.publish
+        if c is not None and c.pcd_save_en and c.interval < 0 and sum(len(a) for a in self.pcd_wait) > 0:
+            self._pcd_write("PCD_all.pcd")
+            self.pcd_wait = []
 
     def world_cloud(self):
         """The undistorted raw cloud of the last process_raw in the world frame with the current state (publish_frame_world with
