@@ -494,21 +494,25 @@ __global__ void __launch_bounds__(256, LI_PLANE_MIN_BLOCKS) k_icp_plane(MapDev M
             float wx, wy, wz;
             li_body_to_world(P, b.x, b.y, b.z, wx, wy, wz);
             if (!SEARCH) S.world[q] = make_float4(wx, wy, wz, 0.f);
-            bool moved = false;
-            if (gate && nb[4].w != 0.f) {
-                if (SEARCH) {
+            const bool fit = gate && nb[4].w != 0.f;
+            if (SEARCH) {
+                // the ordered copies are stored before the plane fit, so that nothing but the fit's own inputs is live across the QR
+                bool moved = false;
+                if (fit) {
                     float d[5];
 #pragma unroll
                     for (int k = 0; k < 5; k++) d[k] = li_dist2(wx, wy, wz, nb[k].x, nb[k].y, nb[k].z);
                     moved = tie_order(nb, d);
                 }
+                if (FROM_IDS || moved) {
+#pragma unroll
+                    for (int k = 0; k < 5; k++) S.near_xyz[(size_t)q * 5 + k] = nb[k];
+                }
+            }
+            if (fit) {
                 float4 nvec;
                 sel = plane_and_row<IMU>(P, b.x, b.y, b.z, wx, wy, wz, nb, nvec, row, r);
                 if (sel) S.normvec[q] = nvec;
-            }
-            if (SEARCH && (FROM_IDS || moved)) {
-#pragma unroll
-                for (int k = 0; k < 5; k++) S.near_xyz[(size_t)q * 5 + k] = nb[k];
             }
             S.selected[q] = sel ? 1 : 0;
         }

@@ -21,7 +21,7 @@
 #include "common.cuh"
 
 #ifndef LI_KNN_U
-#define LI_KNN_U 3           // slab loads issued back to back per lane before the distances are evaluated
+#define LI_KNN_U 2           // slab loads issued back to back per lane before the distances are evaluated (H100 sweep, DESIGN section 3)
 #endif
 #ifndef LI_KNN_THREADS
 #define LI_KNN_THREADS 128
@@ -124,50 +124,60 @@ __device__ __forceinline__ float li_stale_float() {
     return v;
 #endif
 }
+// One buffered candidate: its xyz only. A 128-bit load would tie up the never-read voxel-id word as a fourth register for as long
+// as the candidate waits in the buffer; an 8-byte + a 4-byte load keep three (and measured faster on H100, DESIGN section 3).
+struct LiXyz {
+    float2 xy;
+    float z;
+};
+__device__ __forceinline__ void li_load_xyz(const float4* __restrict__ p, LiXyz& c) {
+    c.xy = __ldg(reinterpret_cast<const float2*>(p));
+    c.z = __ldg(reinterpret_cast<const float*>(p) + 2);
+}
 template <int G, int U = LI_KNN_U>
 __device__ __forceinline__ void group_scan_pipelined(const float4* __restrict__ pool, unsigned f, unsigned cnt, float qx, float qy, float qz,
                                                      float thr, float (&ld)[5], int (&li)[5], int gl) {
     const float cap5 = __uint_as_float(0x40a00001u);   // smallest float above 5: d <= 5 <=> d < cap5
     const float thr5 = fminf(thr, cap5);
     float tau = fminf(thr5, ld[4]);
-    const float4* __restrict__ ptr = pool + f + gl;    // this lane's first candidate of the slab
-    int id = (int)f + gl;
+    const float4* __restrict__ ptr = pool + f + gl;    // this lane's next candidate; the 2U loads of a round use constant offsets from it
     int rem = (int)cnt - gl;                            // candidates left for this lane's column, in units of slab slots
-    float4 a[U], b[U];
+    LiXyz a[U], b[U];
 #pragma unroll
     for (int u = 0; u < U; u++) {   // slots never loaded are never used: their compare is masked by the range test
-        a[u] = make_float4(li_stale_float(), li_stale_float(), li_stale_float(), 0.f);
-        b[u] = make_float4(li_stale_float(), li_stale_float(), li_stale_float(), 0.f);
+        a[u].xy = make_float2(li_stale_float(), li_stale_float());
+        a[u].z = li_stale_float();
+        b[u].xy = make_float2(li_stale_float(), li_stale_float());
+        b[u].z = li_stale_float();
     }
 #pragma unroll
     for (int u = 0; u < U; u++)
-        if (u * G < rem) a[u] = __ldg(ptr + u * G);
+        if (u * G < rem) li_load_xyz(ptr + u * G, a[u]);
     while (__any_sync(LI_FULL, rem > 0)) {
 #pragma unroll
         for (int u = 0; u < U; u++)
-            if ((U + u) * G < rem) b[u] = __ldg(ptr + (U + u) * G);
+            if ((U + u) * G < rem) li_load_xyz(ptr + (U + u) * G, b[u]);
 #pragma unroll
         for (int u = 0; u < U; u++) {
-            float d = li_dist2(qx, qy, qz, a[u].x, a[u].y, a[u].z);
+            float d = li_dist2(qx, qy, qz, a[u].xy.x, a[u].xy.y, a[u].z);
             if (d < tau && u * G < rem) {
-                local_insert(ld, li, d, id + u * G);
+                local_insert(ld, li, d, (int)(ptr - pool) + u * G);   // (the pool offset: only formed for an insert)
                 tau = fminf(thr5, ld[4]);
             }
         }
         if (!__any_sync(LI_FULL, rem > U * G)) break;
 #pragma unroll
         for (int u = 0; u < U; u++)
-            if ((2 * U + u) * G < rem) a[u] = __ldg(ptr + (2 * U + u) * G);
+            if ((2 * U + u) * G < rem) li_load_xyz(ptr + (2 * U + u) * G, a[u]);
 #pragma unroll
         for (int u = 0; u < U; u++) {
-            float d = li_dist2(qx, qy, qz, b[u].x, b[u].y, b[u].z);
+            float d = li_dist2(qx, qy, qz, b[u].xy.x, b[u].xy.y, b[u].z);
             if (d < tau && (U + u) * G < rem) {
-                local_insert(ld, li, d, id + (U + u) * G);
+                local_insert(ld, li, d, (int)(ptr - pool) + (U + u) * G);
                 tau = fminf(thr5, ld[4]);
             }
         }
         ptr += 2 * U * G;
-        id += 2 * U * G;
         rem -= 2 * U * G;
     }
 }
@@ -191,7 +201,7 @@ struct KnnGeom {
 // (Streaming the concatenated slabs through one cursor per group -- no per-brick restart at all -- was measured too and lost to the cursor
 // arithmetic.)
 #ifndef LI_KNN_PB
-#define LI_KNN_PB 2          // bricks evaluated (hash probes in flight) per lane and round; 1, 3 and 4 were slower
+#define LI_KNN_PB 2          // bricks evaluated (hash probes in flight) per lane and round; 1 was slower, 3 no faster on H100
 #endif
 #ifndef LI_KNN_LIST
 #define LI_KNN_LIST 32       // found bricks a group lists before it scans them ...

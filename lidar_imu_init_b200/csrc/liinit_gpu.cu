@@ -404,7 +404,8 @@ void set_scan(Ctx* c, int n) {
 // Lanes per scan point when the caller left knn_group_lanes = 0. A warp works on 32/G points at once and lives as long as its slowest
 // one: 4 lanes give the best throughput once every SM holds several such batches, but a small frame then occupies a fraction of the
 // GPU for a long batch time. The thresholds come from a frame-size sweep of the search kernel (tools/probe_small.py, C2 scene) on the
-// previous target GPU; they have not been re-swept on H100. Every G gives the same neighbours.
+// previous target GPU; one H100 run did not separate them from the alternatives beyond noise (DESIGN section 3). Every G gives the
+// same neighbours.
 int group_for(int n) {
     if (n <= 14000) return 32;
     if (n <= 70000) return 8;
@@ -421,11 +422,16 @@ void attached_slot_read(Ctx* c) {
     else c->attached = nullptr;
 }
 
+#ifndef LI_KNN_WAVES
+#define LI_KNN_WAVES 6   // grid cap of the search kernel in resident waves (H100 sweep, DESIGN section 3: 1, 2, 4 and 8 were slower)
+#endif
 template <int G>
 void launch_knn_scan(Ctx* c, const PoseD& P) {
     long long threads = (long long)c->S.n * G;
     int grid = nblk(threads, LI_KNN_THREADS);
-    int cap = c->max_blocks * (256 / LI_KNN_THREADS);
+    // Large frames: at most LI_KNN_WAVES waves of resident blocks, every warp strides over the query batches. The warps of the
+    // first blocks then take one batch more than the rest and start first, and the blocks that start last are the short ones.
+    const int cap = c->num_sms * LI_KNN_MIN_BLOCKS * LI_KNN_WAVES;
     if (grid > cap) grid = cap;
     // a later search pass of the same scan, no map point removed in between: seeded by the previous pass's neighbours (knn_kernels.cuh)
     const bool seeded = c->have_neighbors && !c->scan_fresh && c->nbr_epoch == c->map_epoch && c->reseed;

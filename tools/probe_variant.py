@@ -1,4 +1,5 @@
-"""One library variant (LIINIT_GPU_LIB), one line: search-kernel ms at both poses of the C2 scene cached in /tmp/c2_probe.npz."""
+"""One library variant (LIINIT_GPU_LIB), one line: search-kernel ms at both poses of the C2 scene cached in /tmp/c2_probe.npz.
+   python tools/probe_variant.py [G]   (G: lanes per point, 0 = group_for's choice)"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
@@ -9,9 +10,10 @@ if not os.path.exists('/tmp/c2_probe.npz'):
     np.savez('/tmp/c2_probe.npz', map=c["map_xyz"], body=c["body_xyz"], init_R=c["pose_init"].rot_end, init_p=c["pose_init"].pos_end,
              gt_R=c["pose_gt"].rot_end, gt_p=c["pose_gt"].pos_end)
 z = np.load('/tmp/c2_probe.npz')
-g = capi.LiInitGpu(0.15, max_map_points=6_000_000, max_scan_points=250_000, knn_index=1)
+G = int(sys.argv[1]) if len(sys.argv) > 1 else 0
+g = capi.LiInitGpu(0.15, max_map_points=6_000_000, max_scan_points=250_000, knn_index=1, knn_group_lanes=G)
 g.map_build(z["map"]); g.scan_upload(z["body"])
-out = [os.path.basename(os.environ.get("LIINIT_GPU_LIB", "default"))]
+out = [os.path.basename(os.environ.get("LIINIT_GPU_LIB", "default")) + f" G={G}"]
 for pose in ("init", "gt"):
     R, p = z[pose + "_R"], z[pose + "_p"]
     I, zero = np.eye(3), np.zeros(3)
