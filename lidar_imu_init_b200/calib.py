@@ -94,6 +94,10 @@ class LiCalib:
     def push_imu(self, omg, acc, t):
         self._ck(self.L.li_calib_push_imu(self.h, _v(omg), _v(acc), float(t)), "push_imu")
 
+    def clear_imu_all(self):
+        """IMU_buffer_clear: drop the IMU samples pushed so far (the node's IMU loop-back)."""
+        self.L.li_calib_clear_imu_all(self.h)
+
     def sizes(self):
         a, i, l = C.c_int(0), C.c_int(0), C.c_int(0)
         self._ck(self.L.li_calib_sizes(self.h, C.byref(a), C.byref(i), C.byref(l)), "sizes")

@@ -1,0 +1,77 @@
+"""Run LI-Init on a recorded ROS1 bag, without ROS:
+
+    python -m lidar_imu_init_b200.run --config avia.yaml --bag rec.bag [--out DIR] [--param name=value ...] [--device N]
+                                      [--max-map-points N]
+
+The config is one of the reference's config/*.yaml as it ships; --param sets a launch-file <param> (point_filter_num, max_iteration,
+cube_side_length) or any other node parameter. Writes DIR/result/Initialization_result.txt, DIR/Log/mat_out.txt,
+DIR/result/trajectory.txt and, with pcd_save_en, DIR/PCD/. Prints print_refine_result's lines on stdout; progress goes to stderr.
+Exits 0 on success, 1 on a bag, message, config or library error, with a message that says what was wrong and where.
+"""
+from __future__ import annotations
+
+import argparse
+import os
+import sys
+import time
+
+from . import config as cfgmod
+from . import rosbag, rosmsg
+
+
+def parse_args(argv=None):
+    ap = argparse.ArgumentParser(prog="python -m lidar_imu_init_b200.run", description=__doc__.split("\n\n")[0],
+                                 formatter_class=argparse.RawDescriptionHelpFormatter)
+    ap.add_argument("--config", required=True, help="a reference config YAML (config/avia.yaml, ouster.yaml, ...)")
+    ap.add_argument("--bag", required=True, help="ROS1 bag (v2.0) with the LiDAR and IMU topics of the config")
+    ap.add_argument("--out", default=".", help="output directory, laid out like the node's package directory (default: .)")
+    ap.add_argument("--param", action="append", default=[], metavar="NAME=VALUE",
+                    help="a node parameter, e.g. max_iteration=5 point_filter_num=2 cube_side_length=2000 (repeatable)")
+    ap.add_argument("--device", type=int, default=0, help="CUDA device (default 0)")
+    ap.add_argument("--max-map-points", type=int, default=6_000_000, help="capacity of the device map (default 6000000)")
+    ap.add_argument("--max-scan-points", type=int, default=300_000, help="capacity of a scan on the device (default 300000)")
+    ap.add_argument("--quiet", action="store_true", help="no progress on stderr")
+    return ap.parse_args(argv)
+
+
+def make_node(args, cfg, log):
+    from . import capi
+    from .node import Node
+    from .odometry import LidarOdometry
+    g = capi.LiInitGpu(cfg.filter_size_map, max_map_points=args.max_map_points, max_scan_points=args.max_scan_points, device_id=args.device)
+    kw = cfgmod.odometry_kwargs(cfg, pcd_dir=os.path.join(args.out, "PCD"))
+    odom = LidarOdometry(g, **kw)
+    return Node(cfg, odom, args.out, log)
+
+
+def main(argv=None, on_node=None) -> int:
+    """The command line; on_node(node), when given, is called with the Node before the bag is played (for tools and tests)."""
+    from . import capi, calib
+    from .node import Log
+    args = parse_args(argv)
+    log = Log(quiet=args.quiet)
+    node = None
+    try:
+        cfg = cfgmod.load(args.config, args.param)
+        with rosbag.Bag(args.bag) as bag:
+            bag.check_topics({cfg.lid_topic: cfgmod.msg_type(cfg), cfg.imu_topic: rosmsg.IMU_TYPE})
+            log.info(f"lidar_type: {cfg.lidar_type} ({cfgmod.LIDAR_NAMES[cfg.lidar_type]}); LiDAR-only odometry starts.")
+            node = make_node(args, cfg, log)
+            if on_node is not None:
+                on_node(node)
+            t0 = time.perf_counter()
+            node.run(bag)
+            wall = time.perf_counter() - t0
+        node.close()
+        node.odom.g.close()
+        log.info(f"{node.updates} updates in {wall:.1f} s; {node.odom.dropped_subframes} sub-frames dropped")
+        return 0
+    except (cfgmod.ConfigError, rosbag.BagError, rosmsg.MsgError, capi.LiInitError, calib.CalibError, OSError) as e:
+        if node is not None and not node.closed:
+            node.close(report=False)
+        sys.stderr.write(f"error: {e}\n")
+        return 1
+
+
+if __name__ == "__main__":
+    sys.exit(main())

@@ -1,0 +1,61 @@
+"""Wall time of a bag replay per recorded second, and the real-time factor, for information only.
+
+    python tools/bag_bench.py --config cfg.yaml --bag rec.bag [--param k=v ...] [--device N]
+    python tools/bag_bench.py --synthetic SECONDS     # writes the 60 s Livox scenario of tests/test_gpu_bag.py (20k points / message)
+
+Prints one JSON line: recorded seconds, wall seconds, wall per recorded second and the real-time factor (recorded / wall; > 1 is
+faster than real time). The bag and the outputs go to a temporary directory.
+"""
+from __future__ import annotations
+
+import argparse
+import json
+import os
+import sys
+import tempfile
+import time
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--config")
+    ap.add_argument("--bag")
+    ap.add_argument("--param", action="append", default=[])
+    ap.add_argument("--device", type=int, default=0)
+    ap.add_argument("--synthetic", type=float, default=0.0, help="seconds of the synthetic Livox scenario")
+    a = ap.parse_args()
+    from lidar_imu_init_b200 import rosbag, run
+    with tempfile.TemporaryDirectory() as tmp:
+        if a.synthetic:
+            import pathlib
+
+            import test_bag_node as tb
+            ev, _ = tb.livox_events(a.synthetic, 20_000)
+            a.bag = os.path.join(tmp, "sim.bag")
+            tb.write_event_bag(a.bag, ev, chunk_msgs=300)
+            tb.sim_config(pathlib.Path(tmp), online_refine_time=10.0)
+            a.config = os.path.join(tmp, "sim.yaml")
+        with rosbag.Bag(a.bag) as b:
+            times = [e[1] for c in b.chunks for e in c.entries]
+        recorded = (max(times) - min(times)) * 1e-9
+        seen = {}
+        argv = ["--config", a.config, "--bag", a.bag, "--out", os.path.join(tmp, "out"), "--device", str(a.device), "--quiet"]
+        for p in a.param:
+            argv += ["--param", p]
+        t0 = time.perf_counter()
+        rc = run.main(argv, on_node=lambda nd: seen.update(node=nd))
+        wall = time.perf_counter() - t0
+    if rc != 0:
+        sys.exit(rc)
+    nd = seen["node"]
+    print(json.dumps(dict(recorded_s=round(recorded, 3), wall_s=round(wall, 3), wall_per_recorded_s=round(wall / recorded, 4),
+                          real_time_factor=round(recorded / wall, 3), updates=nd.updates, dropped_subframes=nd.odom.dropped_subframes,
+                          init_frame=nd.init_scan, refine_frame=nd.refine_scan)))
+
+
+if __name__ == "__main__":
+    main()
