@@ -54,7 +54,7 @@ POINTCLOUD2_FIELDS = (("x", 0, 7, 1), ("y", 4, 7, 1), ("z", 8, 7, 1), ("normal_x
                       ("intensity", 32, 7, 1), ("curvature", 36, 7, 1))
 # Livox CustomPoint: 19 bytes on the wire, 20 as the ROS struct (align=True)
 LIVOX_POINT = np.dtype([("offset_time", "<u4"), ("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("reflectivity", "u1"), ("tag", "u1"), ("line", "u1")])
-LIVOX_POINT_ALIGNED = np.dtype(LIVOX_POINT, align=True)
+LIVOX_POINT_ALIGNED = np.dtype(LIVOX_POINT.descr, align=True)    # (np.dtype(LIVOX_POINT, align=True) would keep 19 bytes)
 
 _f32 = np.ctypeslib.ndpointer(dtype=np.float32, flags="C_CONTIGUOUS")
 _f64 = np.ctypeslib.ndpointer(dtype=np.float64, flags="C_CONTIGUOUS")

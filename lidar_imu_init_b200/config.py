@@ -202,9 +202,11 @@ def check(cfg: Config, where: str):
         raise ConfigError(f"{where}: cut_frame_num, orig_odom_freq, max_iteration and point_filter_num must be positive")
 
 
-def msg_type(cfg: Config) -> str:
+def wanted_topics(cfg: Config, fmt: str) -> dict:
+    """{topic: accepted message types} of the node's LiDAR and IMU subscriptions in a bag of format fmt (rosmsg.decoders)."""
     from . import rosmsg
-    return rosmsg.LIVOX_TYPE if cfg.lidar_type == 1 else rosmsg.PCL2_TYPE
+    d = rosmsg.decoders(fmt, cfg.lidar_type)
+    return {cfg.lid_topic: d.lidar_types, cfg.imu_topic: d.imu_types}
 
 
 def odometry_kwargs(cfg: Config, pcd_dir: str = "PCD") -> dict:

@@ -19,7 +19,7 @@ import sys
 import numpy as np
 
 from . import config as cfgmod
-from . import host, rosbag, rosmsg
+from . import host, rosmsg
 from .odometry import LidarOdometry
 
 
@@ -255,24 +255,24 @@ class Node:
         if not o.imu_en and o.data_accum_start and self.updates % 50 == 0:
             self.log.info("[Initialization] data accumulation, frame %d" % o.frame_num)
 
-    def run(self, bag: rosbag.Bag):
-        """Deliver every message of the configured LiDAR and IMU topics in playback order, each followed by spin()."""
+    def run(self, bag):
+        """Deliver every message of the configured LiDAR and IMU topics in playback order, each followed by spin(). bag: a
+        rosbag.Bag or a rosbag2.Bag2; its `format` picks the decoders (rosmsg.decoders)."""
         c = self.cfg
         if c.lid_topic == c.imu_topic:
             raise cfgmod.ConfigError(f"common/lid_topic and common/imu_topic are both {c.lid_topic!r}")
-        lidar_type = cfgmod.msg_type(c)
-        wanted = {c.lid_topic: lidar_type, c.imu_topic: rosmsg.IMU_TYPE}
+        dec = rosmsg.decoders(bag.format, c.lidar_type)
+        wanted = cfgmod.wanted_topics(c, bag.format)
         total = bag.count(wanted)
-        self.log.info(f"{bag.path}: {total} messages on {c.lid_topic} [{lidar_type}] and {c.imu_topic} [{rosmsg.IMU_TYPE}]")
+        types = bag.topics()
+        self.log.info(f"{bag.path}: {total} messages on {c.lid_topic} [{types[c.lid_topic]}] and {c.imu_topic} [{types[c.imu_topic]}]")
+        lidar_cbk = self.livox_cbk if c.lidar_type == 1 else self.pcl2_cbk
         for i, m in enumerate(bag.messages(wanted)):
             try:
                 if m.topic == c.imu_topic:
-                    self.imu_cbk(*rosmsg.decode_imu(m.data))
-                elif c.lidar_type == 1:
-                    self.livox_cbk(*rosmsg.decode_livox(m.data))
+                    self.imu_cbk(*dec.imu(m.data))
                 else:
-                    stamp, data, lay, n = rosmsg.decode_pcl2(m.data, c.lidar_type)
-                    self.pcl2_cbk(stamp, data, lay, n)
+                    lidar_cbk(*dec.lidar(m.data))
             except rosmsg.MsgError as e:
                 raise rosmsg.MsgError(f"{bag.path}: message {i} on {m.topic} at record time {m.sec}.{m.nsec:09d}: {e}") from None
             self.spin()

@@ -19,6 +19,8 @@ import warnings
 
 import numpy as np
 
+from . import rosmsg
+
 MAGIC = b"#ROSBAG V2.0\n"
 OP_MSG_DATA, OP_BAG_HEADER, OP_INDEX_DATA, OP_CHUNK, OP_CHUNK_INFO, OP_CONNECTION = 0x02, 0x03, 0x04, 0x05, 0x06, 0x07
 
@@ -100,6 +102,7 @@ class _Chunk:
 
 class Bag:
     """bag = Bag(path); bag.topics() -> {topic: type}; for m in bag.messages({topic: (type, ...)}): ..."""
+    format = "ros1"     # the serialization of its messages (rosmsg.decoders)
 
     def __init__(self, path: str):
         self.path = path
@@ -256,7 +259,8 @@ class Bag:
 
     def check_topics(self, wanted: dict) -> dict:
         """wanted {topic: accepted type or tuple of types}. Raises BagError naming the bag's topics for a missing topic or a topic of
-        another type. Returns {conn id: topic} of the chosen connections."""
+        another type, and a livox_ros_driver2/CustomMsg connection whose definition differs from livox_ros_driver/CustomMsg (naming the
+        first field that differs). Returns {conn id: topic} of the chosen connections."""
         out = {}
         for topic, types in wanted.items():
             types = (types,) if isinstance(types, str) else tuple(types)
@@ -267,6 +271,10 @@ class Bag:
                 if c["type"] not in types:
                     raise BagError(f"{self.path}: topic {topic!r} carries {c['type']}, expected {' or '.join(types)}; the bag has: "
                                    f"{self._describe()}")
+                why = rosmsg.definition_mismatch(c["type"], c["message_definition"])
+                if why is not None:
+                    raise BagError(f"{self.path}: topic {topic!r} carries {c['type']}, whose message_definition differs from "
+                                   f"{rosmsg.LIVOX_TYPE}: {why}")
                 out[k] = topic
         return out
 

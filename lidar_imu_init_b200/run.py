@@ -1,7 +1,11 @@
-"""Run LI-Init on a recorded ROS1 bag, without ROS:
+"""Run LI-Init on a recorded ROS1 or ROS 2 bag, without ROS:
 
     python -m lidar_imu_init_b200.run --config avia.yaml --bag rec.bag [--out DIR] [--param name=value ...] [--device N]
                                       [--max-map-points N]
+
+--bag is a ROS1 bag (v2.0), a rosbag2 directory (sqlite3 storage) or one of its .db3 files, told apart by the file's first bytes. The
+LiDAR topic carries livox_ros_driver/CustomMsg or livox_ros_driver2/CustomMsg (lidar_type 1) or sensor_msgs/PointCloud2 in a ROS1
+bag, and livox_ros_driver2/msg/CustomMsg or sensor_msgs/msg/PointCloud2 in a ROS 2 bag.
 
 The config is one of the reference's config/*.yaml as it ships; --param sets a launch-file <param> (point_filter_num, max_iteration,
 cube_side_length) or any other node parameter. Writes DIR/result/Initialization_result.txt, DIR/Log/mat_out.txt,
@@ -16,14 +20,15 @@ import sys
 import time
 
 from . import config as cfgmod
-from . import rosbag, rosmsg
+from . import rosbag, rosbag2, rosmsg
 
 
 def parse_args(argv=None):
     ap = argparse.ArgumentParser(prog="python -m lidar_imu_init_b200.run", description=__doc__.split("\n\n")[0],
                                  formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--config", required=True, help="a reference config YAML (config/avia.yaml, ouster.yaml, ...)")
-    ap.add_argument("--bag", required=True, help="ROS1 bag (v2.0) with the LiDAR and IMU topics of the config")
+    ap.add_argument("--bag", required=True, help="ROS1 bag (v2.0), rosbag2 directory or .db3 file with the LiDAR and IMU topics of "
+                    "the config")
     ap.add_argument("--out", default=".", help="output directory, laid out like the node's package directory (default: .)")
     ap.add_argument("--param", action="append", default=[], metavar="NAME=VALUE",
                     help="a node parameter, e.g. max_iteration=5 point_filter_num=2 cube_side_length=2000 (repeatable)")
@@ -53,8 +58,8 @@ def main(argv=None, on_node=None) -> int:
     node = None
     try:
         cfg = cfgmod.load(args.config, args.param)
-        with rosbag.Bag(args.bag) as bag:
-            bag.check_topics({cfg.lid_topic: cfgmod.msg_type(cfg), cfg.imu_topic: rosmsg.IMU_TYPE})
+        with rosbag2.open_bag(args.bag) as bag:
+            bag.check_topics(cfgmod.wanted_topics(cfg, bag.format))
             log.info(f"lidar_type: {cfg.lidar_type} ({cfgmod.LIDAR_NAMES[cfg.lidar_type]}); LiDAR-only odometry starts.")
             node = make_node(args, cfg, log)
             if on_node is not None:

@@ -1,7 +1,10 @@
 """Wall time of a bag replay per recorded second, and the real-time factor, for information only.
 
     python tools/bag_bench.py --config cfg.yaml --bag rec.bag [--param k=v ...] [--device N]
-    python tools/bag_bench.py --synthetic SECONDS     # writes the 60 s Livox scenario of tests/test_gpu_bag.py (20k points / message)
+    python tools/bag_bench.py --synthetic SECONDS [--ros2]   # writes the Livox scenario of tests/test_gpu_bag.py (20k points / message);
+                                                             # --ros2: as the rosbag2 directory of tests/test_gpu_bag2.py
+
+--bag takes whatever `run --bag` takes: a ROS1 bag, a rosbag2 directory or a .db3 file.
 
 Prints one JSON line: recorded seconds, wall seconds, wall per recorded second and the real-time factor (recorded / wall; > 1 is
 faster than real time). The bag and the outputs go to a temporary directory.
@@ -27,21 +30,35 @@ def main():
     ap.add_argument("--param", action="append", default=[])
     ap.add_argument("--device", type=int, default=0)
     ap.add_argument("--synthetic", type=float, default=0.0, help="seconds of the synthetic Livox scenario")
+    ap.add_argument("--ros2", action="store_true", help="write the synthetic scenario as a ROS 2 bag (livox_ros_driver2/msg/CustomMsg)")
     a = ap.parse_args()
-    from lidar_imu_init_b200 import rosbag, run
+    from lidar_imu_init_b200 import rosbag, rosbag2, run
     with tempfile.TemporaryDirectory() as tmp:
         if a.synthetic:
             import pathlib
 
             import test_bag_node as tb
             ev, _ = tb.livox_events(a.synthetic, 20_000)
-            a.bag = os.path.join(tmp, "sim.bag")
-            tb.write_event_bag(a.bag, ev, chunk_msgs=300)
+            if a.ros2:
+                import test_bag2_node as t2
+                a.bag = os.path.join(tmp, "sim_ros2")
+                t2.write_event_bag2(a.bag, ev, files=3)
+            else:
+                a.bag = os.path.join(tmp, "sim.bag")
+                tb.write_event_bag(a.bag, ev, chunk_msgs=300)
             tb.sim_config(pathlib.Path(tmp), online_refine_time=10.0)
             a.config = os.path.join(tmp, "sim.yaml")
-        with rosbag.Bag(a.bag) as b:
-            times = [e[1] for c in b.chunks for e in c.entries]
-        recorded = (max(times) - min(times)) * 1e-9
+        with rosbag2.open_bag(a.bag) as b:
+            if isinstance(b, rosbag.Bag):
+                times = [e[1] for c in b.chunks for e in c.entries]
+                bounds = (min(times), max(times)) if times else None
+            else:
+                bounds = b.time_bounds()
+            fmt = b.format
+        if bounds is None:
+            sys.exit(f"{a.bag}: the bag holds no messages")
+        t0, t1 = bounds
+        recorded = (t1 - t0) * 1e-9
         seen = {}
         argv = ["--config", a.config, "--bag", a.bag, "--out", os.path.join(tmp, "out"), "--device", str(a.device), "--quiet"]
         for p in a.param:
@@ -52,7 +69,7 @@ def main():
     if rc != 0:
         sys.exit(rc)
     nd = seen["node"]
-    print(json.dumps(dict(recorded_s=round(recorded, 3), wall_s=round(wall, 3), wall_per_recorded_s=round(wall / recorded, 4),
+    print(json.dumps(dict(format=fmt, recorded_s=round(recorded, 3), wall_s=round(wall, 3), wall_per_recorded_s=round(wall / recorded, 4),
                           real_time_factor=round(recorded / wall, 3), updates=nd.updates, dropped_subframes=nd.odom.dropped_subframes,
                           init_frame=nd.init_scan, refine_frame=nd.refine_scan)))
 
