@@ -76,6 +76,10 @@ int li_calib_initialize(li_calib* c, int orig_odom_freq, int cut_frame_num, doub
  *   1: LiDAR_meas.txt  (:151-157)  ang_vel(3) |ang_vel| linear_acc-STD_GRAV(3) ang_acc(3) t   -> 11 columns
  *   2: Lidar_omg_after_rot.txt (:397-400)  R_LI*ang_vel + gyro_bias (3) t                      ->  4 columns
  *   3: acc_cost.txt    (:477-484)  acc_I(3) acc_L(3) t_IMU t_LiDAR                             ->  8 columns
+ *   4: IMU_before_filter.txt   (:43-47)  ang_vel(3) |ang_vel| linear_acc(3) t                  ->  8 columns
+ *   5: Lidar_before_filter.txt (:48-51)  ang_vel(3) |ang_vel| t                                ->  5 columns
+ * Tables 4 and 5 are the IMU / LiDAR groups entering the filters (after downsample_interpolate_IMU, or as loaded with
+ * from_groups), each without its last element, as fout_before_filter writes them.
  * out: row-major [cap_rows x columns]; *rows = rows available. */
 int li_calib_log_rows(const li_calib* c, int which, double* out, int cap_rows, int* rows);
 

@@ -17,7 +17,8 @@ _LIB = None
 SYMBOLS = ["li_calib_create", "li_calib_destroy", "li_calib_set_data_accum_length", "li_calib_set_solver", "li_calib_push_imu_all", "li_calib_push_lidar",
            "li_calib_push_imu", "li_calib_sizes", "li_calib_clear_imu_all", "li_calib_data_sufficiency", "li_calib_initialize",
            "li_calib_log_rows"]
-LOG_COLUMNS = {"IMU_meas": (0, 11), "LiDAR_meas": (1, 11), "Lidar_omg_after_rot": (2, 4), "acc_cost": (3, 8)}
+LOG_COLUMNS = {"IMU_meas": (0, 11), "LiDAR_meas": (1, 11), "Lidar_omg_after_rot": (2, 4), "acc_cost": (3, 8), "IMU_before_filter": (4, 8),
+               "Lidar_before_filter": (5, 5)}
 
 
 class CalibResult(C.Structure):

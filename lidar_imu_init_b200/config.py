@@ -209,15 +209,33 @@ def wanted_topics(cfg: Config, fmt: str) -> dict:
     return {cfg.lid_topic: d.lidar_types, cfg.imu_topic: d.imu_types}
 
 
-def odometry_kwargs(cfg: Config, pcd_dir: str = "PCD") -> dict:
-    """LidarOdometry's constructor arguments (laserMapping.cpp:822-838). Without ROS there is no subscriber for the published clouds:
-    only pcd_save's records are built, and only when pcd_save_en is set. (det_range and cube_side_length are read and checked but
-    LidarOdometry does not segment the map by the field of view.)"""
+# the node's published clouds: LidarOdometry.published key -> topic (laserMapping.cpp:873-878)
+CLOUD_TOPICS = {"registered": "/cloud_registered", "body": "/cloud_registered_body", "effect": "/cloud_effected"}
+# every topic the node publishes a message on (:873-884; /Laser_map has none: publish_map has no caller)
+RECORD_TOPICS = ("/cloud_registered", "/cloud_registered_body", "/cloud_effected", "/aft_mapped_to_init", "/tf", "/path")
+
+
+def odometry_kwargs(cfg: Config, pcd_dir: str = "PCD", record_topics=None) -> dict:
+    """LidarOdometry's constructor arguments (laserMapping.cpp:822-838). Without a recording there is no subscriber for the published
+    clouds: only pcd_save's records are built, and only when pcd_save_en is set. record_topics (the topics a run records, see
+    record_publish) builds the clouds those topics carry. (det_range and cube_side_length are read and checked but LidarOdometry does
+    not segment the map by the field of view.)"""
+    if record_topics is not None:
+        publish = record_publish(cfg, record_topics, pcd_dir)
+    else:
+        publish = dict(scan_pub_en=False, pcd_save_en=True, interval=cfg.interval, pcd_dir=pcd_dir) if cfg.pcd_save_en else None
     return dict(filter_size_map=cfg.filter_size_map, max_iteration=cfg.max_iteration, gyr_cov=cfg.gyr_cov, acc_cov=cfg.acc_cov,
                 orig_odom_freq=cfg.orig_odom_freq, cut_frame_num=cfg.cut_frame_num, data_accum_length=cfg.data_accum_length,
                 filter_size_surf=cfg.filter_size_surf, rot_LI_cov=list(cfg.Rot_LI_cov), trans_LI_cov=list(cfg.Trans_LI_cov),
-                b_gyr_cov=cfg.b_gyr_cov, b_acc_cov=cfg.b_acc_cov, mean_acc_norm=cfg.mean_acc_norm,
-                publish=dict(scan_pub_en=False, pcd_save_en=True, interval=cfg.interval, pcd_dir=pcd_dir) if cfg.pcd_save_en else None)
+                b_gyr_cov=cfg.b_gyr_cov, b_acc_cov=cfg.b_acc_cov, mean_acc_norm=cfg.mean_acc_norm, publish=publish)
+
+
+def record_publish(cfg: Config, topics, pcd_dir: str = "PCD") -> dict:
+    """LidarOdometry's publish= for a run that records the topics `topics`: the node's publish/scan_publish_en, dense_publish_en and
+    scan_bodyframe_pub_en and its pcd_save; a cloud whose topic is not recorded is not downloaded."""
+    return dict(scan_pub_en=cfg.scan_publish_en, dense_pub_en=cfg.dense_publish_en, scan_body_pub_en=cfg.scan_bodyframe_pub_en,
+                pcd_save_en=cfg.pcd_save_en, interval=cfg.interval, pcd_dir=pcd_dir,
+                clouds=tuple(k for k, t in CLOUD_TOPICS.items() if t in topics))
 
 
 def preprocess(cfg: Config) -> dict:

@@ -469,7 +469,7 @@ struct li_calib {
     double lag1 = 0, lag2 = 0, total_lag = 0;
     int lag_frames = 0;
     int solver = 0;   // 0: the reference's ceres-default schedule, 1: Levenberg-Marquardt to convergence
-    std::vector<double> log_rows[4];
+    std::vector<double> log_rows[6];   // li_calib_log_rows: which -> table
 };
 
 namespace {
@@ -724,6 +724,15 @@ int li_calib_initialize(li_calib* c, int orig_odom_freq, int cut_frame_num, doub
         if (c->imu_all.size() < 8 || c->lidar.empty()) return LI_CALIB_ERR_TOO_FEW;
         downsample_interpolate(c, move_start_time);
     }
+    // fout_before_filter (:43-52, :592): the groups as they enter the filters, each without its last element
+    for (size_t i = 0; i + 1 < c->imu.size(); i++) {
+        const Sample& s = c->imu[i];
+        push_row(c->log_rows[4], {s.w.x, s.w.y, s.w.z, s.w.norm(), s.va.x, s.va.y, s.va.z, s.t});
+    }
+    for (size_t i = 0; i + 1 < c->lidar.size(); i++) {
+        const Sample& s = c->lidar[i];
+        push_row(c->log_rows[5], {s.w.x, s.w.y, s.w.z, s.w.norm(), s.t});
+    }
     const size_t need = 2 * kExt + 2 + 10 + 20 + 8;
     if (c->imu.size() < need || c->lidar.size() < need) return LI_CALIB_ERR_TOO_FEW;
     time_compensate(c, 0.0, true);                                       // :592
@@ -845,8 +854,8 @@ int li_calib_initialize(li_calib* c, int orig_odom_freq, int cut_frame_num, doub
 }
 
 int li_calib_log_rows(const li_calib* c, int which, double* out, int cap_rows, int* rows) {
-    if (!c || which < 0 || which > 3 || !rows) return LI_CALIB_ERR_INVALID;
-    static const int cols[4] = {11, 11, 4, 8};
+    if (!c || which < 0 || which > 5 || !rows) return LI_CALIB_ERR_INVALID;
+    static const int cols[6] = {11, 11, 4, 8, 8, 5};
     const std::vector<double>& v = c->log_rows[which];
     const int n = (int)(v.size() / cols[which]);
     *rows = n;

@@ -5,6 +5,9 @@ delivered message, the LI-Init trigger and hand-over, the online-refinement cloc
   <out>/Log/mat_out.txt                    the fout_out row of every update (:1162-1166)
   <out>/result/trajectory.txt              one TUM line per update, the pose of /aft_mapped_to_init (set_posestamp, :647-663)
   <out>/PCD/                               pcd_save (LidarOdometry's Publish path)
+  <out>/Log/<six LI-Init logs>             with open_debug_logs(): LI_Init's logs (LI_init.cpp:11-16), written at the trigger
+
+and, with a Recorder in Node.recorder, the node's published topics in a bag (bagwrite).
 
 Delivery model: after every delivered message the loop body runs until sync_packages has nothing ready (LidarOdometry.process_next
 returns None), i.e. a node that always keeps up with playback (DESIGN §4b). The node's spinOnce batching, which depends on timing, is
@@ -19,7 +22,7 @@ import sys
 import numpy as np
 
 from . import config as cfgmod
-from . import host, rosmsg
+from . import host, pubmsg, rosmsg
 from .odometry import LidarOdometry
 
 
@@ -94,6 +97,29 @@ def state_mat_out_row(state, euler_cur, total_distance) -> str:
                        total_distance)
 
 
+# LI_Init's logs (LI_init.cpp:11-16, in the constructor's order): file -> (calib.LiCalib.log_rows table, the stream's precision,
+# coefficients of each object the row streams: an Eigen row vector (transpose()) or a scalar, separated by one space)
+DEBUG_LOGS = {
+    "LiDAR_meas.txt": ("LiDAR_meas", 12, (3, 1, 3, 3, 1)),                 # :151-156
+    "IMU_meas.txt": ("IMU_meas", 12, (3, 1, 3, 3, 1)),                     # :135-139
+    "IMU_before_filter.txt": ("IMU_before_filter", 15, (3, 1, 3, 1)),      # :45-46
+    "Lidar_before_filter.txt": ("Lidar_before_filter", 15, (3, 1, 1)),     # :49-50
+    "acc_cost.txt": ("acc_cost", 10, (3, 3, 1, 1)),                        # :483-484
+    "Lidar_omg_after_rot.txt": ("Lidar_omg_after_rot", 12, (3, 1)),        # :398-399
+}
+
+
+def log_row(values, precision: int, groups) -> str:
+    """One row of an LI_Init log: the stream's default float format at `precision` significant digits, each Eigen object's
+    coefficients right-aligned to its widest one (eigen_str)."""
+    fmt = lambda v: "%.*g" % (precision, v)   # noqa: E731
+    out, i = [], 0
+    for g in groups:
+        out.append(eigen_str(values[i:i + g], fmt))
+        i += g
+    return " ".join(out) + "\n"
+
+
 def refine_result_lines(state, time_lag) -> list:
     """print_refine_result (laserMapping.cpp:727-743), without the terminal colours."""
     v = state_calib_values(state, time_lag)
@@ -129,6 +155,44 @@ class Log:
         self.info("[WARN] " + msg, "33")
 
 
+class Recorder:
+    """The node's publishers (laserMapping.cpp:561-706) into a bag writer (bagwrite), called after every update with the update's
+    lidar_end_time, the set_posestamp pose and LidarOdometry.published. In the order of the loop (:1137-1157): /aft_mapped_to_init and
+    its /tf transform (publish_odometry), then /cloud_registered, /cloud_registered_body and /cloud_effected as far as they were
+    published, then /path on every 5th call (publish_path's static counter), a growing list of PoseStamped whose header keeps the stamp
+    set once at start-up (:804, lidar_end_time = 0 then). Every other stamp is lidar_end_time, and so is every record time. /Laser_map
+    has no message: publish_map has no caller. Only `topics` are written."""
+    FRAME, CHILD = "camera_init", "aft_mapped"
+
+    def __init__(self, writer, cfg: cfgmod.Config, topics=cfgmod.RECORD_TOPICS):
+        self.w, self.topics, self.path_en = writer, frozenset(topics), cfg.path_en
+        self.path_calls = 0
+        self.path_poses = []
+        self.path_stamp = pubmsg.ros_time(0.0)
+
+    def update(self, t: float, pos, quat, published: dict):
+        stamp, enc, topics, F = pubmsg.ros_time(t), self.w.encoding, self.topics, self.FRAME
+
+        def put(topic, type_, data):
+            self.w.write(topic, type_, stamp, data)
+        if "/aft_mapped_to_init" in topics:
+            put("/aft_mapped_to_init", pubmsg.ODOMETRY, pubmsg.odometry(stamp, F, self.CHILD, pos, quat, enc))
+        if "/tf" in topics:
+            put("/tf", pubmsg.TF_MESSAGE, pubmsg.tf_message(stamp, F, self.CHILD, pos, quat, enc))
+        for key, topic in cfgmod.CLOUD_TOPICS.items():
+            if key in published and topic in topics:
+                put(topic, pubmsg.POINTCLOUD2, pubmsg.pointcloud2(stamp, F, published[key], enc))
+        if self.path_en:
+            self.path_calls += 1
+            if self.path_calls % 5 == 0:
+                self.path_poses.append((stamp, F, tuple(pos), tuple(quat)))
+                if "/path" in topics:
+                    put("/path", pubmsg.PATH, pubmsg.path(self.path_stamp, F, self.path_poses, enc))
+
+    def close(self):
+        self.w.close()
+
+
 class Node:
     """laserMapping's main(): node.imu_cbk / node.livox_cbk / node.pcl2_cbk deliver messages, each followed by node.spin(); node.run(bag)
     does both over a bag; node.close() ends the run (pcd_save's last file, the end-of-run report)."""
@@ -151,7 +215,20 @@ class Node:
         self.init_state = self.refine_state = None  # the states written under "Initialization result:" / "Refinement result:"
         self.updates = 0
         self.on_update = None                       # callback(node) after every update's output rows, for tests and tools
+        self.recorder = None                        # a Recorder: the published topics of every update go to its bag
+        self.debug_logs = None                      # open_debug_logs(): {file name: open file} of LI_Init's logs
         self.closed = False
+
+    def open_debug_logs(self):
+        """Create LI_Init's six logs in <out>/Log/, empty until the trigger writes them (LI_init.cpp:11-16)."""
+        self.debug_logs = {name: open(os.path.join(self.out_dir, "Log", name), "w") for name in DEBUG_LOGS}
+
+    def _write_debug_logs(self):
+        calib = self.odom.calib
+        for name, f in self.debug_logs.items():
+            table, precision, groups = DEBUG_LOGS[name]
+            f.write("".join(log_row(r, precision, groups) for r in calib.log_rows(table)))
+            f.flush()
 
     @property
     def time_lag(self) -> float:
@@ -225,6 +302,8 @@ class Node:
         t = o.lidar_end_time
         self.f_traj.write("%.9f %s %s\n" % (t, " ".join("%.9g" % v for v in pos), " ".join("%.9g" % v for v in q)))
         self.f_mat.write(state_mat_out_row(s, euler_cur, self.total_distance))
+        if self.recorder is not None:
+            self.recorder.update(t, pos, q, o.published)
         if self.on_update is not None:               # the posterior of the update, before the hand-over of a trigger scan
             self.on_update(self)
         # the refinement clock (:1169-1187)
@@ -245,6 +324,8 @@ class Node:
         # the trigger (:1190-1233): LidarOdometry has pushed the scan and assessed the data; LI_Initialization and the hand-over run now
         if not o.imu_en and o.data_accum_finished:
             self.init_result = res = o.initialize(o.imu_buffer.timediff)
+            if self.debug_logs is not None:
+                self._write_debug_logs()
             self.online_calib_starts_time = t
             o.hand_over(res)
             self.init_scan = o.frame_num
@@ -284,8 +365,10 @@ class Node:
             return
         self.closed = True
         self.odom.close()
-        for f in (self.f_result, self.f_mat, self.f_traj):
+        for f in (self.f_result, self.f_mat, self.f_traj, *(self.debug_logs or {}).values()):
             f.close()
+        if self.recorder is not None:
+            self.recorder.close()
         if not report:
             return
         if self.init_result is None:

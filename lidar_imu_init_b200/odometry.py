@@ -36,6 +36,8 @@ class Publish:
     pcd_save_en: bool = False       # pcd_save/pcd_save_en
     interval: int = -1              # pcd_save/interval
     pcd_dir: str = "PCD"
+    # which of the published clouds are built when their condition holds (a recording that does not keep a topic skips its download)
+    clouds: tuple = ("registered", "body", "effect")
 
 
 class ImuBuffer:
@@ -287,21 +289,23 @@ class LidarOdometry:
 
     def _publish(self, R, p, RLI, TLI):
         """The "Publish points" block of the loop (:1152-1156) with the posterior: publish_frame_world (:561-614) when scan_pub_en or
-        pcd_save_en, publish_frame_body (:616-623) when scan_pub_en and scan_body_pub_en, publish_effect_world (:625-636) always.
-        The records land in self.published; pcd_save accumulates the REGISTERED records on the host."""
+        pcd_save_en, publish_frame_body (:616-623) when scan_pub_en and scan_body_pub_en, publish_effect_world (:625-636) always;
+        each only when it is in Publish.clouds. The records land in self.published; pcd_save accumulates the REGISTERED records on the
+        host."""
         c = self.publish
         out = {}
         reg = None
-        if c.scan_pub_en:
+        if c.scan_pub_en and "registered" in c.clouds:
             which = capi.CLOUD_REGISTERED if c.dense_pub_en else capi.CLOUD_REGISTERED_DOWN
             out["registered"] = self.g.cloud(which, R, p, RLI, TLI)
             if c.dense_pub_en:
                 reg = out["registered"]
         if c.pcd_save_en:
             self._pcd_save(reg if reg is not None else self.g.cloud(capi.CLOUD_REGISTERED, R, p, RLI, TLI))
-        if c.scan_pub_en and c.scan_body_pub_en:
+        if c.scan_pub_en and c.scan_body_pub_en and "body" in c.clouds:
             out["body"] = self.g.cloud(capi.CLOUD_BODY)
-        out["effect"] = self.g.cloud(capi.CLOUD_EFFECT, R, p, RLI, TLI)
+        if "effect" in c.clouds:
+            out["effect"] = self.g.cloud(capi.CLOUD_EFFECT, R, p, RLI, TLI)
         self.published = out
 
     def _pcd_save(self, reg):

@@ -170,6 +170,12 @@ def decode_pcl2(buf, lidar_type: int):
 
 # ---- ROS 2 (CDR) ----
 
+def cdr_pad(pos: int, size: int) -> int:
+    """The padding CDR puts before a primitive of `size` bytes at byte `pos` of a message, counted from the message's first byte (the
+    alignment is counted from the byte after the 4-byte encapsulation header). Shared by the decoders and pubmsg's serializers."""
+    return -(pos - 4) % size
+
+
 class _CdrReader(_Reader):
     """CDR little endian after the 4-byte encapsulation header; unpack aligns to the size of the format's last item (every format
     used here has items of one size)."""
@@ -185,7 +191,7 @@ class _CdrReader(_Reader):
             raise MsgError(f"{what}: encapsulation header {head.hex(' ') or '(empty message)'} is not CDR little endian (00 01)")
 
     def align(self, n):
-        self.p += -(self.p - 4) % n
+        self.p += cdr_pad(self.p, n)
 
     def unpack(self, fmt):
         self.align(struct.calcsize("<" + fmt[-1]))

@@ -1,7 +1,8 @@
 """Run LI-Init on a recorded ROS1 or ROS 2 bag, without ROS:
 
     python -m lidar_imu_init_b200.run --config avia.yaml --bag rec.bag [--out DIR] [--param name=value ...] [--device N]
-                                      [--max-map-points N]
+                                      [--max-map-points N] [--record PATH [--record-format ros1|ros2]
+                                      [--record-compression none|bz2] [--record-topics a,b,...]] [--debug-logs]
 
 --bag is a ROS1 bag (v2.0), a rosbag2 directory (sqlite3 storage) or one of its .db3 files, told apart by the file's first bytes. The
 LiDAR topic carries livox_ros_driver/CustomMsg or livox_ros_driver2/CustomMsg (lidar_type 1) or sensor_msgs/PointCloud2 in a ROS1
@@ -11,6 +12,10 @@ The config is one of the reference's config/*.yaml as it ships; --param sets a l
 cube_side_length) or any other node parameter. Writes DIR/result/Initialization_result.txt, DIR/Log/mat_out.txt,
 DIR/result/trajectory.txt and, with pcd_save_en, DIR/PCD/. Prints print_refine_result's lines on stdout; progress goes to stderr.
 Exits 0 on success, 1 on a bag, message, config or library error, with a message that says what was wrong and where.
+
+--record PATH writes the node's published topics (/cloud_registered, /cloud_registered_body, /cloud_effected, /aft_mapped_to_init,
+/tf, /path; --record-topics chooses some) under the node's publish/* parameters into a new bag: a ROS1 bag for a ROS1 input, a rosbag2
+directory for a ROS 2 input, or as --record-format says. --debug-logs writes LI-Init's six logs to DIR/Log/.
 """
 from __future__ import annotations
 
@@ -19,6 +24,7 @@ import os
 import sys
 import time
 
+from . import bagwrite
 from . import config as cfgmod
 from . import rosbag, rosbag2, rosmsg
 
@@ -36,7 +42,27 @@ def parse_args(argv=None):
     ap.add_argument("--max-map-points", type=int, default=6_000_000, help="capacity of the device map (default 6000000)")
     ap.add_argument("--max-scan-points", type=int, default=300_000, help="capacity of a scan on the device (default 300000)")
     ap.add_argument("--quiet", action="store_true", help="no progress on stderr")
+    ap.add_argument("--record", metavar="PATH", help="record the node's published topics into a new bag at PATH")
+    ap.add_argument("--record-format", choices=bagwrite.FORMATS, help="ros1 (a .bag file) or ros2 (a rosbag2 directory); default: "
+                    "the format of --bag")
+    ap.add_argument("--record-compression", choices=bagwrite.COMPRESSIONS, default="none", help="chunk compression of a ROS1 "
+                    "recording (default none)")
+    ap.add_argument("--record-topics", metavar="TOPIC,...", help="the topics to record, comma-separated (default: all of "
+                    + ", ".join(cfgmod.RECORD_TOPICS) + ")")
+    ap.add_argument("--debug-logs", action="store_true", help="write LI-Init's logs (LiDAR_meas.txt, IMU_meas.txt, ...) to DIR/Log/")
     return ap.parse_args(argv)
+
+
+def record_topics(args) -> tuple:
+    """The topics --record-topics names (all the node publishes when it is not given)."""
+    if args.record_topics is None:
+        return cfgmod.RECORD_TOPICS
+    topics = tuple(dict.fromkeys(t.strip() for t in args.record_topics.split(",") if t.strip()))
+    bad = [t for t in topics if t not in cfgmod.RECORD_TOPICS]
+    if bad or not topics:
+        raise cfgmod.ConfigError(f"--record-topics {args.record_topics!r}: {'unknown topic ' + repr(bad[0]) if bad else 'no topic'}; "
+                                 f"the node publishes {', '.join(cfgmod.RECORD_TOPICS)}")
+    return topics
 
 
 def make_node(args, cfg, log):
@@ -44,7 +70,7 @@ def make_node(args, cfg, log):
     from .node import Node
     from .odometry import LidarOdometry
     g = capi.LiInitGpu(cfg.filter_size_map, max_map_points=args.max_map_points, max_scan_points=args.max_scan_points, device_id=args.device)
-    kw = cfgmod.odometry_kwargs(cfg, pcd_dir=os.path.join(args.out, "PCD"))
+    kw = cfgmod.odometry_kwargs(cfg, pcd_dir=os.path.join(args.out, "PCD"), record_topics=record_topics(args) if args.record else None)
     odom = LidarOdometry(g, **kw)
     return Node(cfg, odom, args.out, log)
 
@@ -52,16 +78,24 @@ def make_node(args, cfg, log):
 def main(argv=None, on_node=None) -> int:
     """The command line; on_node(node), when given, is called with the Node before the bag is played (for tools and tests)."""
     from . import capi, calib
-    from .node import Log
+    from .node import Log, Recorder
     args = parse_args(argv)
     log = Log(quiet=args.quiet)
-    node = None
+    node = writer = None
     try:
         cfg = cfgmod.load(args.config, args.param)
+        topics = record_topics(args)
         with rosbag2.open_bag(args.bag) as bag:
             bag.check_topics(cfgmod.wanted_topics(cfg, bag.format))
+            if args.record:
+                fmt = args.record_format or ("ros1" if bag.format == "ros1" else "ros2")
+                writer = bagwrite.open_writer(args.record, fmt, args.record_compression)
             log.info(f"lidar_type: {cfg.lidar_type} ({cfgmod.LIDAR_NAMES[cfg.lidar_type]}); LiDAR-only odometry starts.")
             node = make_node(args, cfg, log)
+            if writer is not None:
+                node.recorder = Recorder(writer, cfg, topics)
+            if args.debug_logs:
+                node.open_debug_logs()
             if on_node is not None:
                 on_node(node)
             t0 = time.perf_counter()
@@ -72,10 +106,20 @@ def main(argv=None, on_node=None) -> int:
         log.info(f"{node.updates} updates in {wall:.1f} s; {node.odom.dropped_subframes} sub-frames dropped")
         return 0
     except (cfgmod.ConfigError, rosbag.BagError, rosmsg.MsgError, capi.LiInitError, calib.CalibError, OSError) as e:
-        if node is not None and not node.closed:
-            node.close(report=False)
+        _abort(node, writer)
         sys.stderr.write(f"error: {e}\n")
         return 1
+    except BaseException:
+        # an interrupted run (Ctrl-C) still closes its files and its recording, so the bag it leaves is complete
+        _abort(node, writer)
+        raise
+
+
+def _abort(node, writer):
+    if node is not None and not node.closed:
+        node.close(report=False)                    # closes the recording too
+    elif node is None and writer is not None:
+        writer.close()
 
 
 if __name__ == "__main__":

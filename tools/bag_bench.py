@@ -4,10 +4,12 @@
     python tools/bag_bench.py --synthetic SECONDS [--ros2]   # writes the Livox scenario of tests/test_gpu_bag.py (20k points / message);
                                                              # --ros2: as the rosbag2 directory of tests/test_gpu_bag2.py
 
---bag takes whatever `run --bag` takes: a ROS1 bag, a rosbag2 directory or a .db3 file.
+--bag takes whatever `run --bag` takes: a ROS1 bag, a rosbag2 directory or a .db3 file. --record also replays the bag a second time
+with `run --record` (every topic the node publishes, in the format of the input) and reports both runs and the recording's size.
 
 Prints one JSON line: recorded seconds, wall seconds, wall per recorded second and the real-time factor (recorded / wall; > 1 is
-faster than real time). The bag and the outputs go to a temporary directory.
+faster than real time); with --record also record_wall_s, record_real_time_factor and record_bytes. The bag and the outputs go to a
+temporary directory.
 """
 from __future__ import annotations
 
@@ -31,6 +33,7 @@ def main():
     ap.add_argument("--device", type=int, default=0)
     ap.add_argument("--synthetic", type=float, default=0.0, help="seconds of the synthetic Livox scenario")
     ap.add_argument("--ros2", action="store_true", help="write the synthetic scenario as a ROS 2 bag (livox_ros_driver2/msg/CustomMsg)")
+    ap.add_argument("--record", action="store_true", help="replay once more with run --record and report both")
     a = ap.parse_args()
     from lidar_imu_init_b200 import rosbag, rosbag2, run
     with tempfile.TemporaryDirectory() as tmp:
@@ -66,12 +69,23 @@ def main():
         t0 = time.perf_counter()
         rc = run.main(argv, on_node=lambda nd: seen.update(node=nd))
         wall = time.perf_counter() - t0
-    if rc != 0:
-        sys.exit(rc)
-    nd = seen["node"]
-    print(json.dumps(dict(format=fmt, recorded_s=round(recorded, 3), wall_s=round(wall, 3), wall_per_recorded_s=round(wall / recorded, 4),
-                          real_time_factor=round(recorded / wall, 3), updates=nd.updates, dropped_subframes=nd.odom.dropped_subframes,
-                          init_frame=nd.init_scan, refine_frame=nd.refine_scan)))
+        if rc != 0:
+            sys.exit(rc)
+        nd = seen["node"]
+        res = dict(format=fmt, recorded_s=round(recorded, 3), wall_s=round(wall, 3), wall_per_recorded_s=round(wall / recorded, 4),
+                   real_time_factor=round(recorded / wall, 3), updates=nd.updates, dropped_subframes=nd.odom.dropped_subframes,
+                   init_frame=nd.init_scan, refine_frame=nd.refine_scan)
+        if a.record:
+            rec = os.path.join(tmp, "recording")
+            argv[argv.index("--out") + 1] = os.path.join(tmp, "out_record")
+            t0 = time.perf_counter()
+            rc = run.main(argv + ["--record", rec])
+            wall_r = time.perf_counter() - t0
+            if rc != 0:
+                sys.exit(rc)
+            size = os.path.getsize(rec) if os.path.isfile(rec) else sum(os.path.getsize(os.path.join(rec, f)) for f in os.listdir(rec))
+            res.update(record_wall_s=round(wall_r, 3), record_real_time_factor=round(recorded / wall_r, 3), record_bytes=size)
+    print(json.dumps(res))
 
 
 if __name__ == "__main__":
