@@ -223,6 +223,44 @@ int liinit_cloud_download(liinit_ctx* h, int which, const double rot_end[9], con
 int liinit_map_incremental(liinit_ctx* h, const double rot_end[9], const double pos_end[3], const double R_LI[9],
                            const double T_LI[3], double ds, int flg_EKF_inited, int* n_add, int* n_no_downsample);
 
+/* ---- device-pointer twins: clouds that are already on the GPU (a PyTorch pipeline, a simulator) ----------------------------------
+ * Each function behaves like its host twin named in its comment -- same arguments, layouts, error codes and results, bit for bit --
+ * except that its point arrays are memory of the context's device instead of host memory.
+ *   Pointers: every point array (input or output) must be cudaMemoryTypeDevice or cudaMemoryTypeManaged memory of the context's
+ *     device (cudaPointerGetAttributes). Otherwise, and for a null array where the twin needs one, the call returns LIINIT_ERR_INVALID,
+ *     liinit_last_error names the argument, and NOTHING changes: map, resident scan, staged cloud and liinit_launch_count are as before.
+ *     A stride-4 input that is 16-byte aligned is read as float4 in place; any other input is repacked from the caller's memory.
+ *   Stream order: the work is queued on the context's stream (liinit_set_stream / liinit_get_stream). An input only has to be ready on
+ *     that stream when the call is made, an output is valid once that stream reaches it, and an input may be reused once that stream
+ *     has passed the call. A call synchronises only where its twin returns a host scalar that the device computes: the map updates
+ *     (capacity errors, `added`), the host count of an EFFECT cloud, and the brick count that sizes a map download.
+ *   With a communicator attached (liinit_comm_init) every device twin returns LIINIT_ERR_INVALID: the device frame is not cut into
+ *   rank slots. */
+/* The stream the context runs on (its own, or the one given to liinit_set_stream), as a cudaStream_t. */
+int liinit_get_stream(liinit_ctx* h, void** cuda_stream);
+/* liinit_map_build: xyz read in place (stride 4, aligned) or repacked on the device. Synchronises once at the end (capacity errors). */
+int liinit_map_build_device(liinit_ctx* h, const float* xyz, int stride_floats, int n);
+/* liinit_map_add_points: *added returned to the host as the twin does (one synchronisation per 2^20-point chunk). */
+int liinit_map_add_points_device(liinit_ctx* h, const float* xyz, int stride_floats, int n, int downsample_on, int* added);
+/* liinit_scan_upload: stride 4 is one device-to-device copy, 3 and 12 are repacked from the caller's memory. No synchronisation. */
+int liinit_scan_upload_device(liinit_ctx* h, const float* body_xyz, int stride_floats, int n);
+/* liinit_raw_upload: repacked from the caller's memory; the PointType layout (stride >= 12, time_index 9) brings normals and intensity
+ * along as the twin does. No synchronisation. */
+int liinit_raw_upload_device(liinit_ctx* h, const float* pts, int stride_floats, int time_index, int n);
+/* liinit_map_nearest_search: queries, out_xyz [n*5*3], out_d2 [n*5] and out_cnt [n] on the device (any output may be NULL). The count
+ * and the PointType_CMP tie order (ikd_Tree.h:57-60, applied when both out_xyz and out_d2 are given) are computed on the device,
+ * exactly as the twin computes them on the host. No synchronisation, any n. */
+int liinit_map_nearest_search_device(liinit_ctx* h, const float* q_xyz, int stride_floats, int n, double max_dist, float* out_xyz,
+                                     float* out_d2, int* out_cnt);
+/* liinit_cloud_download: the records are built in rec12 itself, which must be 16-byte aligned. n (host, may be NULL) and d_n (device,
+ * may be NULL) receive the point count. REGISTERED, BODY and REGISTERED_DOWN never synchronise. EFFECT synchronises only when n is
+ * given or when cap_points is smaller than the resident scan (the count must then be known before anything is written). */
+int liinit_cloud_download_device(liinit_ctx* h, int which, const double rot_end[9], const double pos_end[3], const double R_LI[9],
+                                 const double T_LI[3], float* rec12, int cap_points, int* n, int* d_n);
+/* liinit_map_download: the live points as packed xyz into xyz [cap_points*3], their number into *d_n (device, required; counts past
+ * cap_points are not written, as in the twin). Synchronises once for the brick count that sizes the launch. */
+int liinit_map_download_device(liinit_ctx* h, float* xyz, int cap_points, int* d_n);
+
 /* Test hook: esti_plane<double>(pabcd, points, 0.1) (include/common_lib.h:236-269) of the device for n independent neighbour sets.
  * nb_xyz [n*15] = five xyz per set (f32), pabcd [n*4] = (nx, ny, nz, d), valid [n]. The very function the plane pass calls. */
 int liinit_debug_esti_plane(liinit_ctx* h, const float* nb_xyz, int n, double* pabcd, unsigned char* valid);

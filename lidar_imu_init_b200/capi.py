@@ -3,6 +3,11 @@
 The CUDA library is REQUIRED: importing a handle without the built
 libliinit_gpu.so, or on a machine without a usable GPU, raises -- there is no
 CPU fallback on the product path.
+
+Point arrays may be numpy arrays (the host entry points) or any object with a
+__cuda_array_interface__, such as a torch CUDA tensor or a CuPy array (the
+liinit_*_device twins: read in place on the GPU). Results of device calls are
+torch tensors on the context's device; torch is imported only on those paths.
 """
 from __future__ import annotations
 
@@ -68,6 +73,8 @@ SYMBOLS = [
     "liinit_icp_iterate", "liinit_icp_iterate_device", "liinit_scan_download_effect", "liinit_scan_download_state",
     "liinit_cloud_download", "liinit_map_incremental", "liinit_last_pass_timing", "liinit_last_pass_kernel_times", "liinit_launch_count", "liinit_map_stats", "liinit_knn_index",
     "liinit_comm_unique_id", "liinit_comm_init", "liinit_comm_info", "liinit_comm_last_local", "liinit_comm_mode", "liinit_debug_esti_plane", "liinit_set_reseed",
+    "liinit_get_stream", "liinit_map_build_device", "liinit_map_add_points_device", "liinit_scan_upload_device", "liinit_raw_upload_device",
+    "liinit_map_nearest_search_device", "liinit_cloud_download_device", "liinit_map_download_device",
 ]
 
 
@@ -133,6 +140,14 @@ def load():
     L.liinit_comm_mode.argtypes = [vp, C.POINTER(C.c_int)]
     L.liinit_set_reseed.argtypes = [vp, C.c_int]
     L.liinit_comm_info.argtypes = [vp, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]
+    L.liinit_get_stream.argtypes = [vp, C.POINTER(vp)]
+    L.liinit_map_build_device.argtypes = [vp, vp, C.c_int, C.c_int]
+    L.liinit_map_add_points_device.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int)]
+    L.liinit_scan_upload_device.argtypes = [vp, vp, C.c_int, C.c_int]
+    L.liinit_raw_upload_device.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int]
+    L.liinit_map_nearest_search_device.argtypes = [vp, vp, C.c_int, C.c_int, C.c_double, vp, vp, vp]
+    L.liinit_cloud_download_device.argtypes = [vp, C.c_int, vp, vp, vp, vp, vp, C.c_int, C.POINTER(C.c_int), vp]
+    L.liinit_map_download_device.argtypes = [vp, vp, C.c_int, vp]
     for s in SYMBOLS:
         getattr(L, s).restype = getattr(L, s).restype if s == "liinit_last_error" else C.c_int
     _LIB = L
@@ -151,6 +166,33 @@ def _ptr(a):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
 
 
+def _cai(a):
+    """The __cuda_array_interface__ of a device array, None for anything else (numpy arrays, CPU tensors)."""
+    return getattr(a, "__cuda_array_interface__", None)
+
+
+def _dev_rows(ci, widths):
+    """(pointer, row stride in floats, rows) of a device array of float32 rows, C-contiguous, of one of the given widths."""
+    if np.dtype(ci["typestr"]) != np.float32:
+        raise LiInitError(-1, f"device points must be float32, not {np.dtype(ci['typestr'])}")
+    shape = tuple(ci["shape"])
+    if len(shape) != 2 or not widths(shape[1]):
+        raise LiInitError(-1, f"device points of shape {shape}: the C-ABI takes [n, 3], [n, 4] or [n, 12] rows (raw clouds: [n, >= 3])")
+    st = ci.get("strides")
+    if st is not None and shape[0] > 0 and (st[1] != 4 or (shape[0] > 1 and st[0] != 4 * shape[1])):
+        raise LiInitError(-1, f"device points with byte strides {tuple(st)}: rows must be contiguous float32 (e.g. .contiguous())")
+    return C.c_void_p(ci["data"][0]), shape[1], shape[0]
+
+
+def _xyz_rows(ci):
+    return _dev_rows(ci, lambda w: w in (3, 4, 12))
+
+
+def _torch():
+    import torch
+    return torch
+
+
 class LiInitGpu:
     """One context = one GPU + one device-resident map + one resident scan."""
 
@@ -165,6 +207,8 @@ class LiInitGpu:
             raise LiInitError(rc, (self.L.liinit_last_error(None) or b"").decode())
         self.h = h
         self.scan_n = 0
+        self.device_id = device_id
+        self._tstream = None   # (stream pointer, torch.cuda.ExternalStream) of the context's stream
 
     def close(self):
         if getattr(self, "h", None):
@@ -184,12 +228,69 @@ class LiInitGpu:
     def set_stream(self, cuda_stream: int):
         self._ck(self.L.liinit_set_stream(self.h, C.c_void_p(cuda_stream)))
 
+    def stream(self) -> int:
+        """The cudaStream_t the context runs on (its own, or the one given to set_stream)."""
+        s = C.c_void_p()
+        self._ck(self.L.liinit_get_stream(self.h, C.byref(s)))
+        return s.value or 0
+
+    # ---- device calls: stream handshake with torch ----
+    def _enter(self):
+        """Before a device call: the context's stream waits for what torch's current stream has queued so far (an event, no device-wide
+        synchronise), so a tensor written by torch just before is ready. Without torch or a CUDA device there is nothing to wait for."""
+        try:
+            torch = _torch()
+        except ImportError:
+            return None
+        if not torch.cuda.is_available():
+            return None
+        ptr = self.stream()
+        if self._tstream is None or self._tstream[0] != ptr:
+            self._tstream = (ptr, torch.cuda.ExternalStream(ptr, device=torch.device("cuda", self.device_id)))
+        ours, cur = self._tstream[1], torch.cuda.current_stream(self.device_id)
+        ours.wait_stream(cur)
+        return ours, cur
+
+    @staticmethod
+    def _leave(tok):
+        """After a device call: torch's current stream waits for the context's stream, so results (and the reuse of the inputs' memory
+        by torch's allocator) come after the call's work."""
+        if tok is not None:
+            tok[1].wait_stream(tok[0])
+
+    def _dev_call(self, fn, *args):
+        tok = self._enter()
+        try:
+            self._ck(fn(self.h, *args))
+        finally:
+            self._leave(tok)
+
+    def _empty(self, shape, dtype):
+        torch = _torch()
+        return torch.empty(shape, dtype=getattr(torch, dtype), device=torch.device("cuda", self.device_id))
+
+    @staticmethod
+    def _tptr(t):
+        return C.c_void_p(t.data_ptr()) if t is not None and t.numel() else None
+
     # ---- map ----
     def map_build(self, xyz):
+        ci = _cai(xyz)
+        if ci is not None:
+            self._dev_call(self.L.liinit_map_build_device, *_xyz_rows(ci))
+            return
         a = _pts(xyz)
         self._ck(self.L.liinit_map_build(self.h, _ptr(a), a.shape[1], a.shape[0]))
 
     def map_add_points(self, xyz, downsample_on: bool) -> int:
+        ci = _cai(xyz)
+        if ci is not None:
+            p, stride, n = _xyz_rows(ci)
+            added = C.c_int(0)
+            if n == 0:
+                return 0
+            self._dev_call(self.L.liinit_map_add_points_device, p, stride, n, int(downsample_on), C.byref(added))
+            return added.value
         a = _pts(xyz)
         added = C.c_int(0)
         if a.shape[0] == 0:
@@ -217,7 +318,14 @@ class LiInitGpu:
         self._ck(self.L.liinit_map_size(self.h, C.byref(n)))
         return n.value
 
-    def map_download(self):
+    def map_download(self, device: bool = False):
+        """The live map points as [n, 3] float32: numpy, or with device=True a torch tensor on the context's device."""
+        if device:
+            n = self.map_validnum()
+            out = self._empty((n, 3), "float32")
+            dn = self._empty((1,), "int32")
+            self._dev_call(self.L.liinit_map_download_device, self._tptr(out), n, self._tptr(dn))
+            return out
         n = self.map_validnum()
         out = np.zeros((max(n, 1), 3), np.float32)
         m = C.c_int(0)
@@ -230,6 +338,13 @@ class LiInitGpu:
         return dict(bricks=b.value, hash_slots=s.value, pool_used=pu.value, pool_cap=pc.value)
 
     def nearest_search(self, q, max_dist=5.0):
+        """(xyz [n, 5, 3], d2 [n, 5], cnt [n]): numpy for host queries, torch tensors on the context's device for device queries."""
+        ci = _cai(q)
+        if ci is not None:
+            p, stride, n = _xyz_rows(ci)
+            xyz, d2, cnt = self._empty((n, 5, 3), "float32"), self._empty((n, 5), "float32"), self._empty((n,), "int32")
+            self._dev_call(self.L.liinit_map_nearest_search_device, p, stride, n, max_dist, self._tptr(xyz), self._tptr(d2), self._tptr(cnt))
+            return xyz, d2, cnt
         a = _pts(q)
         n = a.shape[0]
         xyz = np.zeros((n, 5, 3), np.float32)
@@ -240,6 +355,12 @@ class LiInitGpu:
 
     # ---- scan ----
     def scan_upload(self, body):
+        ci = _cai(body)
+        if ci is not None:
+            p, stride, n = _xyz_rows(ci)
+            self._dev_call(self.L.liinit_scan_upload_device, p, stride, n)
+            self.scan_n = n
+            return
         a = _pts(body)
         self._ck(self.L.liinit_scan_upload(self.h, _ptr(a), a.shape[1], a.shape[0]))
         self.scan_n = a.shape[0]
@@ -254,6 +375,12 @@ class LiInitGpu:
 
     # ---- raw-scan front end ----
     def raw_upload(self, pts, time_index: int = -1):
+        ci = _cai(pts)
+        if ci is not None:
+            p, stride, n = _dev_rows(ci, lambda w: w >= 3)
+            self._dev_call(self.L.liinit_raw_upload_device, p, stride, int(time_index), n)
+            self.raw_n = n
+            return
         a = np.ascontiguousarray(pts, dtype=np.float32)
         self._ck(self.L.liinit_raw_upload(self.h, _ptr(a), a.shape[1], int(time_index), a.shape[0]))
         self.raw_n = a.shape[0]
@@ -388,15 +515,21 @@ class LiInitGpu:
         self._ck(self.L.liinit_scan_download_effect(self.h, _ptr(ori), _ptr(nv), n, C.byref(m)))
         return ori[:m.value], nv[:m.value]
 
-    def cloud(self, which: int, rot_end=None, pos_end=None, R_LI=None, T_LI=None):
+    def cloud(self, which: int, rot_end=None, pos_end=None, R_LI=None, T_LI=None, device: bool = False):
         """One of the node's published clouds (CLOUD_*) as [n, 12] float32 pcl::PointXYZINormal records (the PointCloud2 data of
-        POINTCLOUD2_FIELDS). The world-frame clouds need the pose (the posterior the node publishes with); CLOUD_BODY ignores it."""
+        POINTCLOUD2_FIELDS). The world-frame clouds need the pose (the posterior the node publishes with); CLOUD_BODY ignores it.
+        device=True: a torch tensor on the context's device, built there in place."""
         pose = [None] * 4
         if rot_end is not None:
             pose = [np.ascontiguousarray(rot_end, np.float64).reshape(9), np.ascontiguousarray(pos_end, np.float64).reshape(3),
                     np.ascontiguousarray(R_LI, np.float64).reshape(9), np.ascontiguousarray(T_LI, np.float64).reshape(3)]
         args = [_ptr(a) for a in pose]
         n = C.c_int(0)
+        if device:
+            self._dev_call(self.L.liinit_cloud_download_device, int(which), *args, None, 0, C.byref(n), None)
+            out = self._empty((n.value, 12), "float32")
+            self._dev_call(self.L.liinit_cloud_download_device, int(which), *args, self._tptr(out), n.value, C.byref(n), None)
+            return out
         self._ck(self.L.liinit_cloud_download(self.h, int(which), *args, None, 0, C.byref(n)))
         out = np.zeros((n.value, 12), np.float32)
         self._ck(self.L.liinit_cloud_download(self.h, int(which), *args, _ptr(out), n.value, C.byref(n)))

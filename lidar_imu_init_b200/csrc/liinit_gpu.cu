@@ -5,6 +5,9 @@
 #include "../../include/liinit_gpu.h"
 
 #include <cuda_runtime.h>
+#ifdef LI_SIMT_EMUL
+#include "device_memory_emul.h"   // CPU checker only (tests/emul): tells its cudaMalloc memory from host memory
+#endif
 #ifndef LI_SIMT_EMUL
 #include <dlfcn.h>
 #include <nccl.h>   // types only: the library is dlopen()ed when a communicator is asked for (no link-time dependency)
@@ -242,6 +245,63 @@ int stage_points(Ctx* c, const float* xyz, int stride, int n) {
     c->launches++;
     CU(cudaGetLastError());
     return LIINIT_OK;
+}
+
+// ---- the device-pointer twins (liinit_*_device) ----
+bool has_comm(const Ctx* c) {
+#ifndef LI_SIMT_EMUL
+    return c->comm != nullptr;
+#else
+    (void)c;
+    return false;
+#endif
+}
+
+// An argument of a device twin must be device (or managed) memory of the context's device. Checked before anything is changed.
+int check_device_ptr(Ctx* c, const void* p, const char* what) {
+    if (!p) return fail(c, LIINIT_ERR_INVALID, std::string(what) + " is null");
+    cudaPointerAttributes at;
+    if (cudaPointerGetAttributes(&at, p) != cudaSuccess) {
+        cudaGetLastError();
+        return fail(c, LIINIT_ERR_INVALID, std::string(what) + " is not a pointer the CUDA runtime knows");
+    }
+    if (at.type != cudaMemoryTypeDevice && at.type != cudaMemoryTypeManaged)
+        return fail(c, LIINIT_ERR_INVALID, std::string(what) + " is not device memory (the host twin takes host memory)");
+    if (at.device != c->device)
+        return fail(c, LIINIT_ERR_INVALID, std::string(what) + " is memory of device " + std::to_string(at.device) + ", the context runs on device " +
+                                               std::to_string(c->device));
+    return LIINIT_OK;
+}
+
+int device_twin_check(Ctx* c, int stride) {
+    if (has_comm(c)) return fail(c, LIINIT_ERR_INVALID, "the device-pointer entry points do not take a communicator (liinit_comm_init)");
+    if (stride != 3 && stride != 4 && stride != 12) return fail(c, LIINIT_ERR_INVALID, "stride_floats must be 3, 4 or 12");
+    return LIINIT_OK;
+}
+
+bool aligned16(const void* p) { return ((size_t)p & 15) == 0; }
+
+// stage_points for device memory: a 16-byte aligned stride-4 batch is used in place, any other one is repacked into d_stage_pts
+// straight from the caller's memory. *pts: where the batch now is, as float4.
+int stage_points_device(Ctx* c, const float* xyz, int stride, int n, const float4** pts) {
+    if (n > c->stage_pts_cap) return fail(c, LIINIT_ERR_CAPACITY, "batch exceeds staging capacity");
+    c->raw_n = 0;   // as stage_points: the staging buffer is shared with the raw-scan front end
+    if (stride == 4 && aligned16(xyz)) {
+        *pts = reinterpret_cast<const float4*>(xyz);
+        return LIINIT_OK;
+    }
+    k_repack<<<nblk(n, 256), 256, 0, c->stream>>>(xyz, stride, n, c->d_stage_pts);
+    c->launches++;
+    CU(cudaGetLastError());
+    *pts = c->d_stage_pts;
+    return LIINIT_OK;
+}
+
+// the batch of the host (staging copy) or the device twin as float4
+int stage_batch(Ctx* c, const float* xyz, int stride, int n, bool dev, const float4** pts) {
+    if (dev) return stage_points_device(c, xyz, stride, n, pts);
+    *pts = c->d_stage_pts;
+    return stage_points(c, xyz, stride, n);
 }
 
 int fetch_counters(Ctx* c) {
@@ -929,10 +989,17 @@ int liinit_set_stream(liinit_ctx* h, void* cuda_stream) {
     return LIINIT_OK;
 }
 
-int liinit_map_build(liinit_ctx* h, const float* xyz, int stride, int n) {
-    if (!h || (!xyz && n > 0) || n < 0) return LIINIT_ERR_INVALID;
-    Ctx* c = &h->c;
-    CU(cudaSetDevice(c->device));
+int liinit_get_stream(liinit_ctx* h, void** cuda_stream) {
+    if (!h || !cuda_stream) return LIINIT_ERR_INVALID;
+    *cuda_stream = (void*)h->c.stream;
+    return LIINIT_OK;
+}
+
+}  // extern "C"
+
+namespace {
+// liinit_map_build and its device twin (dev: xyz is device memory, checked by the caller)
+int map_build(Ctx* c, const float* xyz, int stride, int n, bool dev) {
     if (n > c->cfg.max_map_points) return fail(c, LIINIT_ERR_CAPACITY, "n exceeds max_map_points");
     c->map_epoch++;
     // KD_TREE::Build replaces the tree (ikd_Tree.cpp:337-339)
@@ -947,16 +1014,37 @@ int liinit_map_build(liinit_ctx* h, const float* xyz, int stride, int n) {
     // (the retained Nearest_Points are copies: a reuse pass / map_incremental after a map change works on them as in the reference)
     for (long long off = 0; off < n; off += c->stage_pts_cap) {
         int m = (int)((n - off < c->stage_pts_cap) ? (n - off) : c->stage_pts_cap);
-        int r = stage_points(c, xyz + (size_t)off * stride, stride, m);
+        const float4* pts = nullptr;
+        int r = stage_batch(c, xyz + (size_t)off * stride, stride, m, dev, &pts);
         if (r) return r;
-        r = plain_insert(c, c->d_stage_pts, m, nullptr, 0);
+        r = plain_insert(c, pts, m, nullptr, 0);
         if (r) return r;
-        // the staging buffers are reused by the next chunk
-        CU(cudaStreamSynchronize(c->stream));
+        // the staging buffers are reused by the next chunk (the host copy is not stream-ordered against the caller's buffer)
+        if (!dev) CU(cudaStreamSynchronize(c->stream));
     }
     int r = fetch_counters(c);
     if (r) return r;
     return check_map_err(c);
+}
+}  // namespace
+
+extern "C" {
+
+int liinit_map_build(liinit_ctx* h, const float* xyz, int stride, int n) {
+    if (!h || (!xyz && n > 0) || n < 0) return LIINIT_ERR_INVALID;
+    Ctx* c = &h->c;
+    CU(cudaSetDevice(c->device));
+    return map_build(c, xyz, stride, n, false);
+}
+
+int liinit_map_build_device(liinit_ctx* h, const float* xyz, int stride, int n) {
+    if (!h || n < 0) return LIINIT_ERR_INVALID;
+    Ctx* c = &h->c;
+    CU(cudaSetDevice(c->device));
+    int r = device_twin_check(c, stride);
+    if (!r && n > 0) r = check_device_ptr(c, xyz, "xyz");
+    if (r) return r;
+    return map_build(c, xyz, stride, n, true);
 }
 
 }  // extern "C"
@@ -1021,10 +1109,11 @@ int liinit_map_compact(liinit_ctx* h) {
     return compact_map(c);
 }
 
-int liinit_map_add_points(liinit_ctx* h, const float* xyz, int stride, int n, int downsample_on, int* added) {
-    if (!h || (!xyz && n > 0) || n < 0) return LIINIT_ERR_INVALID;
-    Ctx* c = &h->c;
-    CU(cudaSetDevice(c->device));
+}  // extern "C"
+
+namespace {
+// liinit_map_add_points and its device twin (dev: xyz is device memory, checked by the caller)
+int map_add_points(Ctx* c, const float* xyz, int stride, int n, int downsample_on, int* added, bool dev) {
     c->map_epoch++;
     {
         int r = maybe_compact(c, n);
@@ -1033,9 +1122,10 @@ int liinit_map_add_points(liinit_ctx* h, const float* xyz, int stride, int n, in
     int total = 0;
     for (long long off = 0; off < n; off += c->stage_pts_cap) {
         int m = (int)((n - off < c->stage_pts_cap) ? (n - off) : c->stage_pts_cap);
-        int r = stage_points(c, xyz + (size_t)off * stride, stride, m);
+        const float4* pts = nullptr;
+        int r = stage_batch(c, xyz + (size_t)off * stride, stride, m, dev, &pts);
         if (r) return r;
-        r = downsample_on ? downsample_insert(c, c->d_stage_pts, m, nullptr, 0) : plain_insert(c, c->d_stage_pts, m, nullptr, 0);
+        r = downsample_on ? downsample_insert(c, pts, m, nullptr, 0) : plain_insert(c, pts, m, nullptr, 0);
         if (r) return r;
         r = fetch_counters(c);
         if (r) return r;
@@ -1045,6 +1135,26 @@ int liinit_map_add_points(liinit_ctx* h, const float* xyz, int stride, int n, in
     }
     if (added) *added = total;
     return LIINIT_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int liinit_map_add_points(liinit_ctx* h, const float* xyz, int stride, int n, int downsample_on, int* added) {
+    if (!h || (!xyz && n > 0) || n < 0) return LIINIT_ERR_INVALID;
+    Ctx* c = &h->c;
+    CU(cudaSetDevice(c->device));
+    return map_add_points(c, xyz, stride, n, downsample_on, added, false);
+}
+
+int liinit_map_add_points_device(liinit_ctx* h, const float* xyz, int stride, int n, int downsample_on, int* added) {
+    if (!h || n < 0) return LIINIT_ERR_INVALID;
+    Ctx* c = &h->c;
+    CU(cudaSetDevice(c->device));
+    int r = device_twin_check(c, stride);
+    if (!r && n > 0) r = check_device_ptr(c, xyz, "xyz");
+    if (r) return r;
+    return map_add_points(c, xyz, stride, n, downsample_on, added, true);
 }
 
 int liinit_map_delete_boxes(liinit_ctx* h, const float* boxes, int nbox, int* deleted) {
@@ -1134,6 +1244,24 @@ int liinit_map_download(liinit_ctx* h, float* xyz, int cap, int* n) {
     return LIINIT_OK;
 }
 
+int liinit_map_download_device(liinit_ctx* h, float* xyz, int cap, int* d_n) {
+    if (!h || cap < 0) return LIINIT_ERR_INVALID;
+    Ctx* c = &h->c;
+    CU(cudaSetDevice(c->device));
+    int r = device_twin_check(c, 3);
+    if (!r) r = check_device_ptr(c, d_n, "d_n");
+    if (!r && cap > 0) r = check_device_ptr(c, xyz, "xyz");
+    if (r) return r;
+    r = fetch_counters(c);   // the brick count sizes the launch
+    if (r) return r;
+    CU(cudaMemsetAsync(d_n, 0, sizeof(int), c->stream));
+    if (c->h_counters[CNT_BRICKS] > 0)
+        k_map_flatten<<<nblk((long long)c->h_counters[CNT_BRICKS] * 32, 256), 256, 0, c->stream>>>(c->M, c->hash_slots, xyz, cap, d_n);
+    c->launches++;
+    CU(cudaGetLastError());
+    return LIINIT_OK;
+}
+
 int liinit_map_nearest_search(liinit_ctx* h, const float* q, int stride, int n, double max_dist, float* out_xyz, float* out_d2,
                               int* out_cnt) {
     if (!h || !q || n < 0) return LIINIT_ERR_INVALID;
@@ -1189,6 +1317,43 @@ int liinit_map_nearest_search(liinit_ctx* h, const float* q, int stride, int n, 
     return LIINIT_OK;
 }
 
+int liinit_map_nearest_search_device(liinit_ctx* h, const float* q, int stride, int n, double max_dist, float* out_xyz, float* out_d2,
+                                     int* out_cnt) {
+    if (!h || n < 0) return LIINIT_ERR_INVALID;
+    Ctx* c = &h->c;
+    if (max_dist != 5.0) return fail(c, LIINIT_ERR_INVALID, "only max_dist = 5 (laserMapping.cpp:980) is supported");
+    CU(cudaSetDevice(c->device));
+    int r = device_twin_check(c, stride);
+    if (!r) r = check_device_ptr(c, q, "q_xyz");
+    if (!r && out_xyz) r = check_device_ptr(c, out_xyz, "out_xyz");
+    if (!r && out_d2) r = check_device_ptr(c, out_d2, "out_d2");
+    if (!r && out_cnt) r = check_device_ptr(c, out_cnt, "out_cnt");
+    if (r) return r;
+    // chunks of the staging capacity, in stream order: the ids go to d_near_ids (a hand-over inside one search pass, free between
+    // passes) and the distances to d_q_d2, both sized for one chunk; k_query_finish writes the caller's buffers
+    for (long long off = 0; off < n; off += c->stage_pts_cap) {
+        const int m = (int)((n - off < c->stage_pts_cap) ? (n - off) : c->stage_pts_cap);
+        const float4* pts = nullptr;
+        r = stage_points_device(c, q + (size_t)off * stride, stride, m, &pts);
+        if (r) return r;
+        if (c->cells) {
+            const int gq = nblk(m, LI_CELLS_THREADS);
+            if (c->cells_search == 1) k_knn_cells_queries<1><<<gq, LI_CELLS_THREADS, 0, c->stream>>>(c->M, pts, m, c->d_near_ids, c->d_q_d2, c->rho2);
+            else if (c->cells_search == 2) k_knn_cells_queries<2><<<gq, LI_CELLS_THREADS, 0, c->stream>>>(c->M, pts, m, c->d_near_ids, c->d_q_d2, c->rho2);
+            else k_knn_cells_queries<3><<<gq, LI_CELLS_THREADS, 0, c->stream>>>(c->M, pts, m, c->d_near_ids, c->d_q_d2, c->rho2);
+        } else {
+            int grid = nblk((long long)m * 8, 256);
+            if (grid > c->max_blocks) grid = c->max_blocks;
+            k_knn_queries<8><<<grid, 256, 0, c->stream>>>(c->M, pts, m, c->d_near_ids, c->d_q_d2, c->rho2);
+        }
+        k_query_finish<<<nblk(m, 256), 256, 0, c->stream>>>(c->M.pool, c->d_near_ids, c->d_q_d2, m, out_xyz ? out_xyz + (size_t)off * 15 : nullptr,
+                                                            out_d2 ? out_d2 + (size_t)off * 5 : nullptr, out_cnt ? out_cnt + off : nullptr);
+        c->launches += 2;
+        CU(cudaGetLastError());
+    }
+    return LIINIT_OK;
+}
+
 int liinit_scan_upload(liinit_ctx* h, const float* body, int stride, int n) {
     if (!h || !body || n <= 0) return LIINIT_ERR_INVALID;
     Ctx* c = &h->c;
@@ -1209,6 +1374,28 @@ int liinit_scan_upload(liinit_ctx* h, const float* body, int stride, int n) {
         return fail(c, LIINIT_ERR_INVALID, "stride_floats must be 3, 4 or 12");
     }
     // new scan: no neighbours, nothing selected (Nearest_Points / point_selected_surf start over at iteration 0)
+    set_scan(c, n);
+    CU(cudaGetLastError());
+    return LIINIT_OK;
+}
+
+int liinit_scan_upload_device(liinit_ctx* h, const float* body, int stride, int n) {
+    if (!h || n <= 0) return LIINIT_ERR_INVALID;
+    Ctx* c = &h->c;
+    CU(cudaSetDevice(c->device));
+    int r = device_twin_check(c, stride);
+    if (!r) r = check_device_ptr(c, body, "body_xyz");
+    if (r) return r;
+    if (n > c->cfg.max_scan_points) return fail(c, LIINIT_ERR_CAPACITY, "n exceeds max_scan_points");
+    if (stride == 4 && aligned16(body)) {
+        CU(cudaMemcpyAsync(c->d_body, body, (size_t)n * 16, cudaMemcpyDeviceToDevice, c->stream));
+    } else {
+        k_repack<<<nblk(n, 256), 256, 0, c->stream>>>(body, stride, n, c->d_body);
+        c->launches++;
+    }
+    c->attached = nullptr;
+    c->attached_slot_done = false;
+    c->body_attr = false;
     set_scan(c, n);
     CU(cudaGetLastError());
     return LIINIT_OK;
@@ -1243,6 +1430,23 @@ int liinit_raw_upload(liinit_ctx* h, const float* pts, int stride, int time_inde
     // the PointType layout (the time in curvature) brings its normals and intensity along; any other layout has none
     c->stage_attr = stride >= 12 && time_index == 9;
     k_repack_t<<<nblk(n, 256), 256, 0, c->stream>>>(c->d_stage_raw, stride, time_index, n, c->d_stage_pts, c->stage_attr ? c->d_stage_attr : nullptr);
+    c->launches++;
+    c->raw_n = n;
+    CU(cudaGetLastError());
+    return LIINIT_OK;
+}
+
+int liinit_raw_upload_device(liinit_ctx* h, const float* pts, int stride, int time_index, int n) {
+    if (!h || n <= 0) return LIINIT_ERR_INVALID;
+    Ctx* c = &h->c;
+    CU(cudaSetDevice(c->device));
+    if (has_comm(c)) return fail(c, LIINIT_ERR_INVALID, "the device-pointer entry points do not take a communicator (liinit_comm_init)");
+    if (stride < 3 || time_index >= stride || (time_index >= 0 && time_index < 3)) return fail(c, LIINIT_ERR_INVALID, "bad stride / time_index");
+    int r = check_device_ptr(c, pts, "pts");
+    if (r) return r;
+    if (n > c->stage_pts_cap || (size_t)n * stride > c->stage_raw_floats) return fail(c, LIINIT_ERR_CAPACITY, "raw cloud exceeds staging capacity");
+    c->stage_attr = stride >= 12 && time_index == 9;
+    k_repack_t<<<nblk(n, 256), 256, 0, c->stream>>>(pts, stride, time_index, n, c->d_stage_pts, c->stage_attr ? c->d_stage_attr : nullptr);
     c->launches++;
     c->raw_n = n;
     CU(cudaGetLastError());
@@ -1647,11 +1851,14 @@ int liinit_scan_download_effect(liinit_ctx* h, float* ori_xyz, float* normvec, i
     return LIINIT_OK;
 }
 
-int liinit_cloud_download(liinit_ctx* h, int which, const double* R, const double* p, const double* RLI, const double* TLI, float* rec12,
-                          int cap, int* n) {
-    if (!h || !n) return LIINIT_ERR_INVALID;
-    Ctx* c = &h->c;
-    CU(cudaSetDevice(c->device));
+}  // extern "C"
+
+namespace {
+// liinit_cloud_download and its device twin. dev: the records are built in rec12 (device memory) itself, d_n (device, may be null)
+// receives the count; n (host) may then be null, and an EFFECT count is only brought to the host when n asks for it or cap_points
+// does not cover the whole resident scan.
+int cloud_download(Ctx* c, int which, const double* R, const double* p, const double* RLI, const double* TLI, float* rec12, int cap, int* n,
+                   int* d_n, bool dev) {
     if (which < LIINIT_CLOUD_REGISTERED || which > LIINIT_CLOUD_EFFECT) return fail(c, LIINIT_ERR_INVALID, "unknown cloud");
     if (which != LIINIT_CLOUD_BODY && (!R || !p || !RLI || !TLI)) return fail(c, LIINIT_ERR_INVALID, "a world-frame cloud needs the pose");
     const bool raw = which == LIINIT_CLOUD_REGISTERED || which == LIINIT_CLOUD_BODY;
@@ -1660,10 +1867,11 @@ int liinit_cloud_download(liinit_ctx* h, int which, const double* R, const doubl
     if (which == LIINIT_CLOUD_EFFECT && !c->have_neighbors) return fail(c, LIINIT_ERR_INVALID, "no ICP pass on the resident scan yet");
     PoseD P;
     if (which != LIINIT_CLOUD_BODY) fill_pose(P, R, p, RLI, TLI);
-    // the records are built in the strided staging buffer (12 floats per point of the staging capacity), free once a cloud is repacked
-    float* out = c->d_stage_raw;
+    // host twin: the records are built in the strided staging buffer (12 floats per point of the staging capacity), free once a cloud
+    // is repacked
+    float* out = dev ? rec12 : c->d_stage_raw;
     const float4* battr = c->body_attr ? c->d_body_attr : nullptr;
-    int m = 0;
+    int m = 0;   // -1: an EFFECT count left on the device (at most scan_n <= cap)
     if (raw) {
         m = c->raw_n;
     } else if (which == LIINIT_CLOUD_REGISTERED_DOWN) {
@@ -1679,13 +1887,21 @@ int liinit_cloud_download(liinit_ctx* h, int which, const double* R, const doubl
         k_rs_scan<<<1, 1024, 0, c->stream>>>(nb + 1, c->d_vg_block);
         c->launches += 2;
         CU(cudaGetLastError());
-        CU(cudaMemcpyAsync(&m, c->d_vg_block + nb, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-        CU(cudaStreamSynchronize(c->stream));
+        if (d_n) CU(cudaMemcpyAsync(d_n, c->d_vg_block + nb, sizeof(int), cudaMemcpyDeviceToDevice, c->stream));
+        if (n || (rec12 && cap < c->scan_n)) {
+            CU(cudaMemcpyAsync(&m, c->d_vg_block + nb, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+            CU(cudaStreamSynchronize(c->stream));
+        } else {
+            m = -1;
+        }
     }
-    *n = m;
-    if (!rec12) return LIINIT_OK;
-    if (cap < m) return fail(c, LIINIT_ERR_CAPACITY, "cap_points is smaller than the cloud");
-    if (m == 0) return LIINIT_OK;
+    if (n) *n = m;
+    if (rec12 && cap < m) return fail(c, LIINIT_ERR_CAPACITY, "cap_points is smaller than the cloud");
+    if (d_n && which != LIINIT_CLOUD_EFFECT) {
+        k_store_int<<<1, 32, 0, c->stream>>>(d_n, m);
+        c->launches++;
+    }
+    if (!rec12 || m == 0) return LIINIT_OK;
     if (!raw) materialize_scan(c);   // (an attached host scan: the whole frame into d_body)
     const float4* sattr = c->stage_attr ? c->d_stage_attr : nullptr;
     switch (which) {
@@ -1696,9 +1912,35 @@ int liinit_cloud_download(liinit_ctx* h, int which, const double* R, const doubl
     }
     c->launches++;
     CU(cudaGetLastError());
+    if (dev) return LIINIT_OK;
     CU(cudaMemcpyAsync(rec12, out, (size_t)m * 12 * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
     return LIINIT_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int liinit_cloud_download(liinit_ctx* h, int which, const double* R, const double* p, const double* RLI, const double* TLI, float* rec12,
+                          int cap, int* n) {
+    if (!h || !n) return LIINIT_ERR_INVALID;
+    Ctx* c = &h->c;
+    CU(cudaSetDevice(c->device));
+    return cloud_download(c, which, R, p, RLI, TLI, rec12, cap, n, nullptr, false);
+}
+
+int liinit_cloud_download_device(liinit_ctx* h, int which, const double* R, const double* p, const double* RLI, const double* TLI, float* rec12,
+                                 int cap, int* n, int* d_n) {
+    if (!h) return LIINIT_ERR_INVALID;
+    Ctx* c = &h->c;
+    CU(cudaSetDevice(c->device));
+    int r = device_twin_check(c, 12);
+    if (!r && !n && !d_n) r = fail(c, LIINIT_ERR_INVALID, "neither n nor d_n is given");
+    if (!r && d_n) r = check_device_ptr(c, d_n, "d_n");
+    if (!r && rec12) r = check_device_ptr(c, rec12, "rec12");
+    if (!r && rec12 && !aligned16(rec12)) r = fail(c, LIINIT_ERR_INVALID, "rec12 must be 16-byte aligned");
+    if (r) return r;
+    return cloud_download(c, which, R, p, RLI, TLI, rec12, cap, n, d_n, true);
 }
 
 int liinit_map_incremental(liinit_ctx* h, const double* R, const double* p, const double* RLI, const double* TLI, double ds,

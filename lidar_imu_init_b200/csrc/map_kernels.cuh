@@ -733,6 +733,55 @@ __global__ void k_gather_xyz(const float4* __restrict__ pool, const int* __restr
     out[3 * i + 2] = q.z;
 }
 
+// liinit_map_nearest_search_device, per query: the ids and distances k_knn_queries / k_knn_cells_queries left -> the caller's
+// buffers (any may be null). Count and tie order are the host twin's loop restated: the count is the number of ids >= 0, and with
+// both xyz and d2 wanted, four passes over the found ranks [0, cnt) swap neighbours whose distances differ by less than 1e-10 to
+// smaller x first (PointType_CMP, ikd_Tree.h:57-60). (tie_order of the plane kernel bubbles over all five ranks with shrinking
+// bounds; the bounds here follow the host twin, so that the two give the same points bit for bit.)
+__global__ void k_query_finish(const float4* __restrict__ pool, const int* __restrict__ ids, const float* __restrict__ d2, int n,
+                               float* __restrict__ out_xyz, float* __restrict__ out_d2, int* __restrict__ out_cnt) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    float x[5], y[5], z[5], d[5];
+    int cnt = 0;
+#pragma unroll
+    for (int k = 0; k < 5; k++) {
+        const int id = ids[(size_t)i * 5 + k];
+        const float4 q = (id >= 0) ? pool[id] : make_float4(0.f, 0.f, 0.f, 0.f);
+        x[k] = q.x; y[k] = q.y; z[k] = q.z;
+        d[k] = d2[(size_t)i * 5 + k];
+        if (id >= 0) cnt++;
+    }
+    if (out_xyz && out_d2) {
+#pragma unroll
+        for (int pass = 0; pass < 4; pass++) {
+#pragma unroll
+            for (int k = 0; k < 4; k++) {
+                if (k + 1 < cnt && fabsf(d[k] - d[k + 1]) < 1e-10f && x[k + 1] < x[k]) {
+                    float t = x[k]; x[k] = x[k + 1]; x[k + 1] = t;
+                    t = y[k]; y[k] = y[k + 1]; y[k + 1] = t;
+                    t = z[k]; z[k] = z[k + 1]; z[k + 1] = t;
+                    t = d[k]; d[k] = d[k + 1]; d[k + 1] = t;
+                }
+            }
+        }
+    }
+    if (out_cnt) out_cnt[i] = cnt;
+#pragma unroll
+    for (int k = 0; k < 5; k++) {
+        if (out_xyz) {
+            float* o = out_xyz + ((size_t)i * 5 + k) * 3;
+            o[0] = x[k]; o[1] = y[k]; o[2] = z[k];
+        }
+        if (out_d2) out_d2[(size_t)i * 5 + k] = d[k];
+    }
+}
+
+// stores one int in stream order (the point count of a device cloud download)
+__global__ void k_store_int(int* __restrict__ p, int v) {
+    if (blockIdx.x == 0 && threadIdx.x == 0) *p = v;
+}
+
 // ---- flatten -------------------------------------------------------------------------------------
 __global__ void k_map_flatten(MapDev M, unsigned slots, float* __restrict__ out, int cap, int* __restrict__ out_n) {
     int wb = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
