@@ -314,6 +314,56 @@ int liinit_launch_count(liinit_ctx* h, long long* launches);
 /* Map statistics: bricks in use, hash slots, pool points in use / capacity. */
 int liinit_map_stats(liinit_ctx* h, int* bricks, int* hash_slots, long long* pool_used, long long* pool_cap);
 
+/* map assessment (DESIGN.md section 4d) ----------------------------------------------------------------------------------------------
+ * Scores an extrinsic by how sharp a map it builds. The store holds staged (undistorted, body-frame) clouds with the pose and extrinsic
+ * of their update. An evaluation places every stored point with li_body_to_world (fp64, f32 store) using its scan's rot_end / pos_end
+ * and either the scan's own extrinsic (as_run) or a candidate (R_LI, T_LI). Every s-th stored point is a query. Its neighbourhood is
+ * every stored point with d2 <= r2, d2 = ((dx*dx + dy*dy) + dz*dz) of the fp64 offsets; the query itself is included. The fp64 moments
+ * of the offsets give Sigma = S2/n - m m^T. With n >= min_neighbors and det Sigma > 0 the query is valid:
+ * h = 1/2 (3 ln(2 pi e) + ln det Sigma), v = lambda_min(Sigma). Otherwise it is sparse (n < min_neighbors) or degenerate (det <= 0).
+ * MME = mean h and MPV = mean v over the valid queries. Moments are summed in a fixed candidate order and the totals in query order,
+ * so an evaluation is bit-identical from call to call and independent of the launch shape and the SM count.
+ * Every call returns LIINIT_ERR_INVALID, and changes nothing, before liinit_assess_reserve and under a communicator. */
+#define LIINIT_ASSESS_MAX_QUERIES 2000000    /* queries per evaluation; the automatic stride is the smallest that stays within it */
+#define LIINIT_ASSESS_MAX_POINTS (1ll << 30)
+#define LIINIT_ASSESS_MAX_SCANS (1 << 24)
+typedef struct {
+    double radius;        /* r [m], > 0 and finite */
+    int min_neighbors;    /* n_min, >= 4 */
+    int query_stride;     /* s; 0 = automatic */
+    int as_run;           /* 1: every scan with its own stored extrinsic; R_LI / T_LI may then be NULL */
+    int reserved;
+} liinit_assess_params;
+typedef struct {
+    long long points;     /* stored points placed */
+    long long queries;
+    int stride;           /* s used */
+    int scans;            /* stored scans */
+    long long valid, sparse, degenerate;
+    double mme, mpv;      /* NaN when no query is valid */
+} liinit_assess_result;
+/* Allocates the store (max_points points, max_scans scans) and the evaluation buffers, about 110 bytes per point. Calling it again
+ * clears the store. LIINIT_ERR_INVALID for max_points outside [1, LIINIT_ASSESS_MAX_POINTS] or max_scans outside
+ * [1, LIINIT_ASSESS_MAX_SCANS]. */
+int liinit_assess_reserve(liinit_ctx* h, long long max_points, int max_scans);
+/* Appends the staged cloud (the BODY cloud of liinit_cloud_download) with its update's pose and extrinsic: a device-to-device copy, no
+ * synchronisation. When the store has no room for it, nothing is stored, the scan is counted as skipped and *appended = 0
+ * (LIINIT_OK). LIINIT_ERR_INVALID when no raw cloud is staged. */
+int liinit_assess_append(liinit_ctx* h, const double rot_end[9], const double pos_end[3], const double R_LI[9], const double T_LI[3],
+                         int* appended);
+/* Stored points and scans, and scans skipped for lack of room (any pointer may be NULL). */
+int liinit_assess_info(liinit_ctx* h, long long* points, int* scans, int* skipped);
+/* One evaluation (synchronises). Leaves the map, the staged cloud, the resident scan and the ICP state untouched.
+ * LIINIT_ERR_INVALID: radius <= 0 or not finite, min_neighbors < 4, query_stride < 0, an empty store, a non-finite or missing
+ * candidate. LIINIT_ERR_CAPACITY: more than LIINIT_ASSESS_MAX_QUERIES queries for the given stride, or a placed point that is not
+ * finite, lies 2^30 cells or more from the origin, or makes the cloud span more cells than a 63-bit key holds. */
+int liinit_assess_evaluate(liinit_ctx* h, const liinit_assess_params* p, const double R_LI[9], const double T_LI[3], liinit_assess_result* out);
+/* Per-query values of the last evaluation, in query order (query j is stored point j * stride): h, v (NaN for a sparse or degenerate
+ * query) and the neighbour count. *n = queries; any output may be NULL; LIINIT_ERR_CAPACITY when cap < queries. */
+int liinit_assess_download(liinit_ctx* h, double* h_out, double* v_out, int* n_out, long long cap, long long* n);
+/* Test hook: the points the last evaluation placed, xyz [cap*3] in stored order. *n = their number; xyz may be NULL. */
+int liinit_assess_download_placed(liinit_ctx* h, float* xyz, long long cap, long long* n);
+
 #ifdef __cplusplus
 }
 #endif

@@ -42,6 +42,18 @@ class Pcl2Layout(C.Structure):   # liinit_pcl2_layout
                 ("off_ring", C.c_int)]
 
 
+class AssessParams(C.Structure):   # liinit_assess_params
+    _fields_ = [("radius", C.c_double), ("min_neighbors", C.c_int), ("query_stride", C.c_int), ("as_run", C.c_int), ("reserved", C.c_int)]
+
+
+class AssessResult(C.Structure):   # liinit_assess_result
+    _fields_ = [("points", C.c_longlong), ("queries", C.c_longlong), ("stride", C.c_int), ("scans", C.c_int), ("valid", C.c_longlong),
+                ("sparse", C.c_longlong), ("degenerate", C.c_longlong), ("mme", C.c_double), ("mpv", C.c_double)]
+
+
+ASSESS_MAX_QUERIES = 2_000_000   # LIINIT_ASSESS_MAX_QUERIES
+
+
 class SubFrame(C.Structure):   # liinit_subframe
     _fields_ = [("handle", C.c_longlong), ("t_beg", C.c_double), ("end_ms", C.c_float), ("n", C.c_int)]
 
@@ -75,6 +87,8 @@ SYMBOLS = [
     "liinit_comm_unique_id", "liinit_comm_init", "liinit_comm_info", "liinit_comm_last_local", "liinit_comm_mode", "liinit_debug_esti_plane", "liinit_set_reseed",
     "liinit_get_stream", "liinit_map_build_device", "liinit_map_add_points_device", "liinit_scan_upload_device", "liinit_raw_upload_device",
     "liinit_map_nearest_search_device", "liinit_cloud_download_device", "liinit_map_download_device",
+    "liinit_assess_reserve", "liinit_assess_append", "liinit_assess_info", "liinit_assess_evaluate", "liinit_assess_download",
+    "liinit_assess_download_placed",
 ]
 
 
@@ -148,10 +162,24 @@ def load():
     L.liinit_map_nearest_search_device.argtypes = [vp, vp, C.c_int, C.c_int, C.c_double, vp, vp, vp]
     L.liinit_cloud_download_device.argtypes = [vp, C.c_int, vp, vp, vp, vp, vp, C.c_int, C.POINTER(C.c_int), vp]
     L.liinit_map_download_device.argtypes = [vp, vp, C.c_int, vp]
+    set_assess_argtypes(L)
     for s in SYMBOLS:
         getattr(L, s).restype = getattr(L, s).restype if s == "liinit_last_error" else C.c_int
     _LIB = L
     return L
+
+
+def set_assess_argtypes(L):
+    """argtypes of the liinit_assess_* entry points on a loaded library"""
+    vp = C.c_void_p
+    L.liinit_assess_reserve.argtypes = [vp, C.c_longlong, C.c_int]
+    L.liinit_assess_append.argtypes = [vp, _f64, _f64, _f64, _f64, C.POINTER(C.c_int)]
+    L.liinit_assess_info.argtypes = [vp, C.POINTER(C.c_longlong), C.POINTER(C.c_int), C.POINTER(C.c_int)]
+    L.liinit_assess_evaluate.argtypes = [vp, C.POINTER(AssessParams), vp, vp, C.POINTER(AssessResult)]
+    L.liinit_assess_download.argtypes = [vp, vp, vp, vp, C.c_longlong, C.POINTER(C.c_longlong)]
+    L.liinit_assess_download_placed.argtypes = [vp, vp, C.c_longlong, C.POINTER(C.c_longlong)]
+    for s in ("reserve", "append", "info", "evaluate", "download", "download_placed"):
+        getattr(L, "liinit_assess_" + s).restype = C.c_int
 
 
 def _pts(a):
@@ -596,6 +624,52 @@ class LiInitGpu:
         a, b, c, d = C.c_int(), C.c_int(), C.c_int(), C.c_int()
         self._ck(self.L.liinit_comm_info(self.h, C.byref(a), C.byref(b), C.byref(c), C.byref(d)))
         return dict(nranks=a.value, rank=b.value, shard_lo=c.value, shard_n=d.value)
+
+    # ---- map assessment (DESIGN §4d) ----
+    def assess_reserve(self, max_points: int, max_scans: int):
+        """Allocate (or clear) the store of LIO scans and the evaluation buffers."""
+        self._ck(self.L.liinit_assess_reserve(self.h, int(max_points), int(max_scans)))
+
+    def assess_append(self, rot_end, pos_end, R_LI, T_LI) -> bool:
+        """Store the staged cloud with its update's pose and extrinsic; False when the store had no room (the scan is counted as
+        skipped)."""
+        ok = C.c_int(0)
+        self._ck(self.L.liinit_assess_append(self.h, np.ascontiguousarray(rot_end, np.float64).reshape(9), np.ascontiguousarray(pos_end, np.float64).reshape(3),
+                                             np.ascontiguousarray(R_LI, np.float64).reshape(9), np.ascontiguousarray(T_LI, np.float64).reshape(3),
+                                             C.byref(ok)))
+        return bool(ok.value)
+
+    def assess_info(self) -> dict:
+        p, s, k = C.c_longlong(0), C.c_int(0), C.c_int(0)
+        self._ck(self.L.liinit_assess_info(self.h, C.byref(p), C.byref(s), C.byref(k)))
+        return dict(points=p.value, scans=s.value, skipped=k.value)
+
+    def assess_evaluate(self, R_LI=None, T_LI=None, radius: float = 0.3, min_neighbors: int = 10, query_stride: int = 0,
+                        as_run: bool = False) -> dict:
+        """One evaluation of the stored scans with the candidate extrinsic (as_run: each scan's own). Returns the liinit_assess_result
+        fields as a dict."""
+        P = AssessParams(float(radius), int(min_neighbors), int(query_stride), int(bool(as_run)), 0)
+        R = None if R_LI is None else np.ascontiguousarray(R_LI, np.float64).reshape(9)
+        T = None if T_LI is None else np.ascontiguousarray(T_LI, np.float64).reshape(3)
+        out = AssessResult()
+        self._ck(self.L.liinit_assess_evaluate(self.h, C.byref(P), _ptr(R), _ptr(T), C.byref(out)))
+        return {k: getattr(out, k) for k, _ in AssessResult._fields_}
+
+    def assess_download(self):
+        """(h, v, n) of every query of the last evaluation: float64, float64 (NaN when sparse or degenerate), int32."""
+        q = C.c_longlong(0)
+        self._ck(self.L.liinit_assess_download(self.h, None, None, None, 0, C.byref(q)))
+        h, v, n = np.zeros(q.value), np.zeros(q.value), np.zeros(q.value, np.int32)
+        self._ck(self.L.liinit_assess_download(self.h, _ptr(h), _ptr(v), _ptr(n), q.value, C.byref(q)))
+        return h, v, n
+
+    def assess_placed(self):
+        """The stored points as the last evaluation placed them, [n, 3] float32 in stored order."""
+        m = C.c_longlong(0)
+        self._ck(self.L.liinit_assess_download_placed(self.h, None, 0, C.byref(m)))
+        out = np.zeros((m.value, 3), np.float32)
+        self._ck(self.L.liinit_assess_download_placed(self.h, _ptr(out), m.value, C.byref(m)))
+        return out
 
     def knn_index(self) -> int:
         """1 = LIINIT_KNN_BRICKS (lockstep groups over whole bricks), 2 = LIINIT_KNN_CELLS (cell directory, thread per point)."""

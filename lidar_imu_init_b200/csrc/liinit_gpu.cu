@@ -30,6 +30,7 @@
 #include "undistort_kernels.cuh"
 #include "preprocess_kernels.cuh"
 #include "output_kernels.cuh"
+#include "assess_kernels.cuh"
 
 #ifndef LI_CELLS_MINB
 #define LI_CELLS_MINB 6
@@ -200,6 +201,39 @@ struct Ctx {
     bool cells_refresh_warp = true;   // directory refresh: warp per brick (false: thread per brick, the version the CPU checker runs)
     bool cells = false;   // knn_index = LIINIT_KNN_CELLS: per-brick cell directory + thread-per-point search (cells.cuh)
     float rho2 = 0.09f;   // squared seed radius of the 5-NN search
+    // map assessment (liinit_assess_*, assess_kernels.cuh): the stored scans and the buffers of an evaluation, allocated by
+    // liinit_assess_reserve
+    struct Assess {
+        long long cap = 0;   // points (0: not reserved)
+        int max_scans = 0;
+        long long n = 0;     // stored points
+        int scans = 0, skipped = 0;
+        long long last_q = -1;   // queries of the last evaluation (-1: none since the reserve) ...
+        long long last_n = 0;    // ... and the stored points it placed
+        float4* pts = nullptr;   // stored body points, w = scan index
+        PoseD* poses = nullptr;
+        float4* world = nullptr;   // placed points, stored order
+        float4* sorted = nullptr;  // placed points in cell order, w = stored index
+        unsigned long long* key = nullptr;
+        unsigned long long* skey = nullptr;
+        unsigned* k[2] = {nullptr, nullptr};
+        unsigned* v[2] = {nullptr, nullptr};
+        int* hist = nullptr;
+        int* tc = nullptr;   // per-block counts: cell starts, queries, tasks
+        int* tq = nullptr;
+        int* tt = nullptr;
+        int* cell_start = nullptr;
+        unsigned long long* cell_key = nullptr;
+        int* cell_q0 = nullptr;
+        int* qlist = nullptr;
+        int4* tasks = nullptr;
+        int* qn = nullptr;
+        double* qh = nullptr;
+        double* qv = nullptr;
+        int* box = nullptr;
+        AsTotals* tot = nullptr;
+        unsigned* ticket = nullptr;
+    } A;
 };
 
 #define CU(call)                                                                                     \
@@ -749,6 +783,15 @@ const FrameSub* frame_lookup(Ctx* c, long long handle, int* slot) {
     return &c->fr_slot_sub[s][k];
 }
 
+void assess_free(Ctx* c) {
+    Ctx::Assess& A = c->A;
+    cudaFree(A.pts); cudaFree(A.poses); cudaFree(A.world); cudaFree(A.sorted); cudaFree(A.key); cudaFree(A.skey);
+    cudaFree(A.k[0]); cudaFree(A.k[1]); cudaFree(A.v[0]); cudaFree(A.v[1]); cudaFree(A.hist); cudaFree(A.tc); cudaFree(A.tq); cudaFree(A.tt);
+    cudaFree(A.cell_start); cudaFree(A.cell_key); cudaFree(A.cell_q0); cudaFree(A.qlist); cudaFree(A.tasks); cudaFree(A.qn); cudaFree(A.qh);
+    cudaFree(A.qv); cudaFree(A.box); cudaFree(A.tot); cudaFree(A.ticket);
+    A = Ctx::Assess{};
+}
+
 }  // namespace
 
 struct liinit_ctx {
@@ -972,6 +1015,7 @@ int liinit_destroy(liinit_ctx* h) {
 #endif
     cudaFree(c->d_partials); cudaFree(c->d_done); cudaFreeHost(c->h_out); cudaFree(c->d_q_d2);
     frame_free(c);
+    assess_free(c);
     if (c->ev0) cudaEventDestroy(c->ev0);
     if (c->ev1) cudaEventDestroy(c->ev1);
     if (c->evm) cudaEventDestroy(c->evm);
@@ -2199,6 +2243,249 @@ int liinit_knn_index(liinit_ctx* h, int* knn_index) {
 int liinit_launch_count(liinit_ctx* h, long long* launches) {
     if (!h || !launches) return LIINIT_ERR_INVALID;
     *launches = h->c.launches;
+    return LIINIT_OK;
+}
+
+}  // extern "C"
+
+// ---- map assessment (assess_kernels.cuh, DESIGN.md section 4d) ----
+namespace {
+
+int assess_check(Ctx* c) {
+    if (has_comm(c)) return fail(c, LIINIT_ERR_INVALID, "the map assessment does not take a communicator (liinit_comm_init)");
+    if (c->A.cap == 0) return fail(c, LIINIT_ERR_INVALID, "no assessment store (liinit_assess_reserve)");
+    return LIINIT_OK;
+}
+
+// one stable 8-bit pass of the radix sort over A.k[cur] / A.v[cur] into the other buffers
+int assess_sort_pass(Ctx* c, int& cur, int n, int shift) {
+    Ctx::Assess& A = c->A;
+    const int ntiles = nblk(n, RS_TILE);
+    k_rs_hist<<<nblk(ntiles, 4), 128, 0, c->stream>>>(A.k[cur], n, shift, ntiles, A.hist);
+    k_rs_scan<<<1, 1024, 0, c->stream>>>(256 * ntiles, A.hist);
+    k_rs_scatter<<<nblk(ntiles, 4), 128, 0, c->stream>>>(A.k[cur], A.v[cur], n, shift, ntiles, A.hist, A.k[cur ^ 1], A.v[cur ^ 1]);
+    c->launches += 3;
+    CU(cudaGetLastError());
+    cur ^= 1;
+    return LIINIT_OK;
+}
+
+int assess_evaluate(Ctx* c, const liinit_assess_params* prm, const double* R_LI, const double* T_LI, liinit_assess_result* out) {
+    Ctx::Assess& A = c->A;
+    const double r = prm->radius;
+    if (!std::isfinite(r) || !(r > 0.0)) return fail(c, LIINIT_ERR_INVALID, "radius must be positive and finite");
+    if (prm->min_neighbors < 4) return fail(c, LIINIT_ERR_INVALID, "min_neighbors must be at least 4");
+    if (prm->query_stride < 0) return fail(c, LIINIT_ERR_INVALID, "query_stride must be >= 0 (0: automatic)");
+    if (!prm->as_run && (!R_LI || !T_LI)) return fail(c, LIINIT_ERR_INVALID, "a candidate extrinsic needs R_LI and T_LI (or as_run)");
+    if (!prm->as_run)
+        for (int k = 0; k < 12; k++)
+            if (!std::isfinite(k < 9 ? R_LI[k] : T_LI[k - 9])) return fail(c, LIINIT_ERR_INVALID, "R_LI / T_LI must be finite");
+    if (A.n == 0) return fail(c, LIINIT_ERR_INVALID, "the assessment store is empty (liinit_assess_append)");
+    const int n = (int)A.n;
+    const long long s = prm->query_stride > 0 ? prm->query_stride : (A.n + LIINIT_ASSESS_MAX_QUERIES - 1) / LIINIT_ASSESS_MAX_QUERIES;
+    const long long nq = (A.n + s - 1) / s;
+    if (nq > LIINIT_ASSESS_MAX_QUERIES)
+        return fail(c, LIINIT_ERR_CAPACITY, "query_stride gives " + std::to_string(nq) + " queries, more than LIINIT_ASSESS_MAX_QUERIES");
+    PoseD cand{};
+    if (!prm->as_run) {
+        memcpy(cand.RLI, R_LI, 72);
+        memcpy(cand.TLI, T_LI, 24);
+    }
+    const double edge = r * (1.0 + ldexp(1.0, -20));
+    int box[8] = {0x7fffffff, 0x7fffffff, 0x7fffffff, -0x7fffffff - 1, -0x7fffffff - 1, -0x7fffffff - 1, 0, 0};
+    CU(cudaMemcpyAsync(A.box, box, sizeof(box), cudaMemcpyHostToDevice, c->stream));
+    k_as_place<<<nblk(n, 256), 256, 0, c->stream>>>(A.pts, A.poses, n, prm->as_run ? 1 : 0, cand, edge, A.world, A.box);
+    c->launches++;
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(box, A.box, sizeof(box), cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    if (box[6]) return fail(c, LIINIT_ERR_CAPACITY, "a placed point is not finite or lies 2^30 cells or more from the origin");
+    AsGrid G;
+    G.edge = edge;
+    for (int a = 0; a < 3; a++) {
+        G.lo[a] = box[a];
+        G.ext[a] = (long long)box[3 + a] - box[a] + 1;
+    }
+    if ((double)G.ext[0] * (double)G.ext[1] * (double)G.ext[2] > 9.0e18)
+        return fail(c, LIINIT_ERR_CAPACITY, "the placed cloud spans more cells than a 63-bit cell key holds");
+    const unsigned long long cells = (unsigned long long)G.ext[0] * (unsigned long long)G.ext[1] * (unsigned long long)G.ext[2];
+    int bits = 0;
+    while (bits < 64 && ((cells - 1) >> bits)) bits++;
+    k_as_key<<<nblk(n, 256), 256, 0, c->stream>>>(A.world, n, G, A.key, A.k[0], A.v[0]);
+    c->launches++;
+    CU(cudaGetLastError());
+    // stable sort by cell key: the low word's digits, then (keys wider than 32 bits) the high word's; only the digits the box needs
+    int cur = 0;
+    for (int sh = 0; sh < bits && sh < 32; sh += 8) {
+        const int rc = assess_sort_pass(c, cur, n, sh);
+        if (rc) return rc;
+    }
+    if (bits > 32) {
+        k_rs_gather_hi<<<nblk(n, 256), 256, 0, c->stream>>>(A.key, A.v[cur], n, A.k[cur]);
+        c->launches++;
+        for (int sh = 0; sh < bits - 32; sh += 8) {
+            const int rc = assess_sort_pass(c, cur, n, sh);
+            if (rc) return rc;
+        }
+    }
+    k_as_gather<<<nblk(n, 256), 256, 0, c->stream>>>(A.world, A.key, A.v[cur], n, A.sorted, A.skey);
+    c->launches++;
+    const int nb = nblk(n, LI_FR_TILE);
+    const int qs = (int)s;
+    k_as_mark<<<nb, LI_FR_TILE, 0, c->stream>>>(A.skey, A.sorted, n, qs, A.tc, A.tq);
+    k_rs_scan<<<1, 1024, 0, c->stream>>>(nb + 1, A.tc);
+    k_rs_scan<<<1, 1024, 0, c->stream>>>(nb + 1, A.tq);
+    k_as_index<<<nb, LI_FR_TILE, 0, c->stream>>>(A.skey, A.sorted, n, qs, A.tc, A.tq, A.cell_start, A.cell_key, A.cell_q0, A.qlist);
+    // (there are at most n cells: nb blocks cover them)
+    k_as_task_count<<<nb, LI_FR_TILE, 0, c->stream>>>(A.cell_q0, A.tc + nb, A.tt);
+    k_rs_scan<<<1, 1024, 0, c->stream>>>(nb + 1, A.tt);
+    k_as_task_emit<<<nb, LI_FR_TILE, 0, c->stream>>>(A.cell_q0, A.tc + nb, A.tt, A.tasks);
+    c->launches += 8;
+    CU(cudaGetLastError());
+    CU(cudaMemsetAsync(A.ticket, 0, sizeof(unsigned), c->stream));
+    k_as_moments<<<c->num_sms * 8, LI_AS_BLOCK, 0, c->stream>>>(A.sorted, A.cell_start, A.cell_key, A.tc + nb, A.qlist, A.tasks, A.tt + nb, A.ticket,
+                                                                G, r * r, qs, prm->min_neighbors, A.qn, A.qh, A.qv);
+    k_as_reduce<<<1, 1024, 0, c->stream>>>(A.qn, A.qh, A.qv, (int)nq, prm->min_neighbors, A.tot);
+    c->launches += 2;
+    CU(cudaGetLastError());
+    AsTotals T;
+    CU(cudaMemcpyAsync(&T, A.tot, sizeof(T), cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    A.last_q = nq;
+    A.last_n = A.n;
+    out->points = A.n;
+    out->queries = nq;
+    out->stride = qs;
+    out->scans = A.scans;
+    out->valid = T.valid;
+    out->sparse = T.sparse;
+    out->degenerate = T.degenerate;
+    out->mme = T.valid ? T.sum_h / (double)T.valid : NAN;
+    out->mpv = T.valid ? T.sum_v / (double)T.valid : NAN;
+    return LIINIT_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int liinit_assess_reserve(liinit_ctx* h, long long max_points, int max_scans) {
+    if (!h) return LIINIT_ERR_INVALID;
+    Ctx* c = &h->c;
+    if (has_comm(c)) return fail(c, LIINIT_ERR_INVALID, "the map assessment does not take a communicator (liinit_comm_init)");
+    if (max_points < 1 || max_points > LIINIT_ASSESS_MAX_POINTS) return fail(c, LIINIT_ERR_INVALID, "max_points must be in [1, LIINIT_ASSESS_MAX_POINTS]");
+    if (max_scans < 1 || max_scans > LIINIT_ASSESS_MAX_SCANS) return fail(c, LIINIT_ERR_INVALID, "max_scans must be in [1, LIINIT_ASSESS_MAX_SCANS]");
+    CU(cudaSetDevice(c->device));
+    CU(cudaStreamSynchronize(c->stream));
+    assess_free(c);
+    Ctx::Assess& A = c->A;
+    const size_t N = (size_t)max_points, Q = (size_t)(max_points < LIINIT_ASSESS_MAX_QUERIES ? max_points : LIINIT_ASSESS_MAX_QUERIES);
+    const size_t NB = N / LI_FR_TILE + 2;
+    bool ok = cudaMalloc(&A.pts, N * sizeof(float4)) == cudaSuccess && cudaMalloc(&A.poses, (size_t)max_scans * sizeof(PoseD)) == cudaSuccess &&
+              cudaMalloc(&A.world, N * sizeof(float4)) == cudaSuccess && cudaMalloc(&A.sorted, N * sizeof(float4)) == cudaSuccess &&
+              cudaMalloc(&A.key, N * 8) == cudaSuccess && cudaMalloc(&A.skey, N * 8) == cudaSuccess && cudaMalloc(&A.k[0], N * 4) == cudaSuccess &&
+              cudaMalloc(&A.k[1], N * 4) == cudaSuccess && cudaMalloc(&A.v[0], N * 4) == cudaSuccess && cudaMalloc(&A.v[1], N * 4) == cudaSuccess &&
+              cudaMalloc(&A.hist, (N / RS_TILE + 2) * 256 * 4) == cudaSuccess && cudaMalloc(&A.tc, NB * 4) == cudaSuccess &&
+              cudaMalloc(&A.tq, NB * 4) == cudaSuccess && cudaMalloc(&A.tt, NB * 4) == cudaSuccess && cudaMalloc(&A.cell_start, (N + 1) * 4) == cudaSuccess &&
+              cudaMalloc(&A.cell_key, N * 8) == cudaSuccess && cudaMalloc(&A.cell_q0, (N + 1) * 4) == cudaSuccess && cudaMalloc(&A.qlist, Q * 4) == cudaSuccess &&
+              cudaMalloc(&A.tasks, Q * sizeof(int4)) == cudaSuccess && cudaMalloc(&A.qn, Q * 4) == cudaSuccess && cudaMalloc(&A.qh, Q * 8) == cudaSuccess &&
+              cudaMalloc(&A.qv, Q * 8) == cudaSuccess && cudaMalloc(&A.box, 8 * 4) == cudaSuccess && cudaMalloc(&A.tot, sizeof(AsTotals)) == cudaSuccess &&
+              cudaMalloc(&A.ticket, sizeof(unsigned)) == cudaSuccess;
+    if (!ok) {
+        cudaGetLastError();
+        assess_free(c);
+        return fail(c, LIINIT_ERR_CUDA, "cudaMalloc of the assessment store (" + std::to_string(max_points) + " points) failed");
+    }
+    A.cap = max_points;
+    A.max_scans = max_scans;
+    return LIINIT_OK;
+}
+
+int liinit_assess_append(liinit_ctx* h, const double rot_end[9], const double pos_end[3], const double R_LI[9], const double T_LI[3],
+                         int* appended) {
+    if (!h) return LIINIT_ERR_INVALID;
+    Ctx* c = &h->c;
+    if (!rot_end || !pos_end || !R_LI || !T_LI || !appended) return fail(c, LIINIT_ERR_INVALID, "null argument");
+    int r = assess_check(c);
+    if (r) return r;
+    if (c->raw_n <= 0) return fail(c, LIINIT_ERR_INVALID, "no raw cloud staged (liinit_raw_upload / liinit_frame_stage)");
+    CU(cudaSetDevice(c->device));
+    Ctx::Assess& A = c->A;
+    if (A.n + c->raw_n > A.cap || A.scans >= A.max_scans) {
+        A.skipped++;
+        *appended = 0;
+        return LIINIT_OK;
+    }
+    PoseD P;
+    fill_pose(P, rot_end, pos_end, R_LI, T_LI);
+    k_as_store<<<nblk(c->raw_n, 256), 256, 0, c->stream>>>(c->d_stage_pts, c->raw_n, A.scans, P, A.pts + A.n, A.poses);
+    c->launches++;
+    CU(cudaGetLastError());
+    A.n += c->raw_n;
+    A.scans++;
+    *appended = 1;
+    return LIINIT_OK;
+}
+
+int liinit_assess_info(liinit_ctx* h, long long* points, int* scans, int* skipped) {
+    if (!h) return LIINIT_ERR_INVALID;
+    Ctx* c = &h->c;
+    int r = assess_check(c);
+    if (r) return r;
+    if (points) *points = c->A.n;
+    if (scans) *scans = c->A.scans;
+    if (skipped) *skipped = c->A.skipped;
+    return LIINIT_OK;
+}
+
+int liinit_assess_evaluate(liinit_ctx* h, const liinit_assess_params* p, const double R_LI[9], const double T_LI[3], liinit_assess_result* out) {
+    if (!h) return LIINIT_ERR_INVALID;
+    Ctx* c = &h->c;
+    if (!p || !out) return fail(c, LIINIT_ERR_INVALID, "null argument");
+    int r = assess_check(c);
+    if (r) return r;
+    CU(cudaSetDevice(c->device));
+    return assess_evaluate(c, p, R_LI, T_LI, out);
+}
+
+int liinit_assess_download(liinit_ctx* h, double* h_out, double* v_out, int* n_out, long long cap, long long* n) {
+    if (!h) return LIINIT_ERR_INVALID;
+    Ctx* c = &h->c;
+    if (!n) return fail(c, LIINIT_ERR_INVALID, "null argument");
+    int r = assess_check(c);
+    if (r) return r;
+    const long long q = c->A.last_q;
+    if (q < 0) return fail(c, LIINIT_ERR_INVALID, "no evaluation since the store was reserved (liinit_assess_evaluate)");
+    *n = q;
+    if ((h_out || v_out || n_out) && cap < q) return fail(c, LIINIT_ERR_CAPACITY, "cap is smaller than the number of queries");
+    CU(cudaSetDevice(c->device));
+    if (h_out) CU(cudaMemcpyAsync(h_out, c->A.qh, (size_t)q * 8, cudaMemcpyDeviceToHost, c->stream));
+    if (v_out) CU(cudaMemcpyAsync(v_out, c->A.qv, (size_t)q * 8, cudaMemcpyDeviceToHost, c->stream));
+    if (n_out) CU(cudaMemcpyAsync(n_out, c->A.qn, (size_t)q * 4, cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    return LIINIT_OK;
+}
+
+int liinit_assess_download_placed(liinit_ctx* h, float* xyz, long long cap, long long* n) {
+    if (!h) return LIINIT_ERR_INVALID;
+    Ctx* c = &h->c;
+    if (!n) return fail(c, LIINIT_ERR_INVALID, "null argument");
+    int r = assess_check(c);
+    if (r) return r;
+    if (c->A.last_q < 0) return fail(c, LIINIT_ERR_INVALID, "no evaluation since the store was reserved (liinit_assess_evaluate)");
+    const long long m = c->A.last_n;
+    *n = m;
+    if (!xyz) return LIINIT_OK;
+    if (cap < m) return fail(c, LIINIT_ERR_CAPACITY, "cap is smaller than the number of stored points");
+    CU(cudaSetDevice(c->device));
+    std::vector<float4> w((size_t)m);
+    CU(cudaMemcpyAsync(w.data(), c->A.world, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    for (long long i = 0; i < m; i++) {
+        xyz[3 * i] = w[i].x;
+        xyz[3 * i + 1] = w[i].y;
+        xyz[3 * i + 2] = w[i].z;
+    }
     return LIINIT_OK;
 }
 

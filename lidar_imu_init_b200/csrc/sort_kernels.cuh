@@ -91,6 +91,15 @@ __global__ void k_rs_scatter(const unsigned* __restrict__ keys, const unsigned* 
     }
 }
 
+// 64-bit keys (the cell keys of the map assessment, assess_kernels.cuh): the passes above run over the low words with the element
+// index as the value, then this kernel fetches each element's high word by the carried index and the passes run again over the high
+// words. Every pass is stable, so the result is ordered by (high word, low word, index).
+__global__ void k_rs_gather_hi(const unsigned long long* __restrict__ keys64, const unsigned* __restrict__ vals, int n,
+                               unsigned* __restrict__ keys_out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) keys_out[i] = (unsigned)(keys64[vals[i]] >> 32);
+}
+
 // variants whose element count lives in device memory (the voxel grid learns the number of leaves on the device)
 __global__ void k_rs_hist_dev(const unsigned* __restrict__ keys, const int* __restrict__ n_dev, int shift, int ntiles, int* __restrict__ hist) {
     __shared__ int s_cnt[4][256];

@@ -7,7 +7,8 @@ delivered message, the LI-Init trigger and hand-over, the online-refinement cloc
   <out>/PCD/                               pcd_save (LidarOdometry's Publish path)
   <out>/Log/<six LI-Init logs>             with open_debug_logs(): LI_Init's logs (LI_init.cpp:11-16), written at the trigger
 
-and, with a Recorder in Node.recorder, the node's published topics in a bag (bagwrite).
+and, with a Recorder in Node.recorder, the node's published topics in a bag (bagwrite); with an Assessment in Node.assess, the LIO
+scans it scores the calibration on (assess).
 
 Delivery model: after every delivered message the loop body runs until sync_packages has nothing ready (LidarOdometry.process_next
 returns None), i.e. a node that always keeps up with playback (DESIGN §4b). The node's spinOnce batching, which depends on timing, is
@@ -216,6 +217,7 @@ class Node:
         self.updates = 0
         self.on_update = None                       # callback(node) after every update's output rows, for tests and tools
         self.recorder = None                        # a Recorder: the published topics of every update go to its bag
+        self.assess = None                          # an assess.Assessment: every LIO update but the switch scan stores its cloud
         self.debug_logs = None                      # open_debug_logs(): {file name: open file} of LI_Init's logs
         self.closed = False
 
@@ -304,6 +306,9 @@ class Node:
         self.f_mat.write(state_mat_out_row(s, euler_cur, self.total_distance))
         if self.recorder is not None:
             self.recorder.update(t, pos, q, o.published)
+        # (the switch scan re-filters the previous scan's cloud; LiDAR-only updates have no extrinsic in the model)
+        if self.assess is not None and o.imu_en and o.switch_scan != o.frame_num - 1:
+            self.assess.append(R, p, RLI, TLI)
         if self.on_update is not None:               # the posterior of the update, before the hand-over of a trigger scan
             self.on_update(self)
         # the refinement clock (:1169-1187)

@@ -3,6 +3,7 @@
     python -m lidar_imu_init_b200.run --config avia.yaml --bag rec.bag [--out DIR] [--param name=value ...] [--device N]
                                       [--max-map-points N] [--record PATH [--record-format ros1|ros2]
                                       [--record-compression none|bz2] [--record-topics a,b,...]] [--debug-logs]
+                                      [--assess [--assess-radius R] [--assess-max-points N]]
 
 --bag is a ROS1 bag (v2.0), a rosbag2 directory (sqlite3 storage) or one of its .db3 files, told apart by the file's first bytes. The
 LiDAR topic carries livox_ros_driver/CustomMsg or livox_ros_driver2/CustomMsg (lidar_type 1) or sensor_msgs/PointCloud2 in a ROS1
@@ -16,6 +17,9 @@ Exits 0 on success, 1 on a bag, message, config or library error, with a message
 --record PATH writes the node's published topics (/cloud_registered, /cloud_registered_body, /cloud_effected, /aft_mapped_to_init,
 /tf, /path; --record-topics chooses some) under the node's publish/* parameters into a new bag: a ROS1 bag for a ROS1 input, a rosbag2
 directory for a ROS 2 input, or as --record-format says. --debug-logs writes LI-Init's six logs to DIR/Log/.
+
+--assess stores the LIO scans on the device and, at the end of the run, scores the calibration by how sharp a map it builds: the mean
+map entropy and plane variance of the as-run, final and perturbed extrinsics, written to DIR/result/assessment.txt (assess).
 """
 from __future__ import annotations
 
@@ -24,6 +28,7 @@ import os
 import sys
 import time
 
+from . import assess as assessmod
 from . import bagwrite
 from . import config as cfgmod
 from . import rosbag, rosbag2, rosmsg
@@ -50,6 +55,12 @@ def parse_args(argv=None):
     ap.add_argument("--record-topics", metavar="TOPIC,...", help="the topics to record, comma-separated (default: all of "
                     + ", ".join(cfgmod.RECORD_TOPICS) + ")")
     ap.add_argument("--debug-logs", action="store_true", help="write LI-Init's logs (LiDAR_meas.txt, IMU_meas.txt, ...) to DIR/Log/")
+    ap.add_argument("--assess", action="store_true", help="score the calibration by the sharpness of the map of the LIO scans: "
+                    "DIR/result/assessment.txt")
+    ap.add_argument("--assess-radius", type=float, default=assessmod.RADIUS, metavar="R",
+                    help=f"neighbourhood radius of the assessment [m] (default {assessmod.RADIUS:g})")
+    ap.add_argument("--assess-max-points", type=int, default=assessmod.MAX_POINTS, metavar="N",
+                    help=f"LIO points the assessment stores on the device (default {assessmod.MAX_POINTS}); later scans are skipped")
     return ap.parse_args(argv)
 
 
@@ -85,6 +96,10 @@ def main(argv=None, on_node=None) -> int:
     try:
         cfg = cfgmod.load(args.config, args.param)
         topics = record_topics(args)
+        if args.assess and not (args.assess_radius > 0 and args.assess_radius < float("inf")):
+            raise cfgmod.ConfigError(f"--assess-radius {args.assess_radius!r}: must be a positive number of metres")
+        if args.assess and args.assess_max_points < 1:
+            raise cfgmod.ConfigError(f"--assess-max-points {args.assess_max_points}: must be positive")
         with rosbag2.open_bag(args.bag) as bag:
             bag.check_topics(cfgmod.wanted_topics(cfg, bag.format))
             if args.record:
@@ -96,12 +111,18 @@ def main(argv=None, on_node=None) -> int:
                 node.recorder = Recorder(writer, cfg, topics)
             if args.debug_logs:
                 node.open_debug_logs()
+            if args.assess:
+                node.assess = assessmod.Assessment(node.odom.g, args.assess_max_points, args.assess_radius)
             if on_node is not None:
                 on_node(node)
             t0 = time.perf_counter()
             node.run(bag)
             wall = time.perf_counter() - t0
         node.close()
+        if node.assess is not None:
+            t0 = time.perf_counter()
+            node.assess.write(os.path.join(args.out, "result", "assessment.txt"))
+            log.info(f"assessment written to {os.path.join(args.out, 'result', 'assessment.txt')} in {time.perf_counter() - t0:.1f} s")
         node.odom.g.close()
         log.info(f"{node.updates} updates in {wall:.1f} s; {node.odom.dropped_subframes} sub-frames dropped")
         return 0
