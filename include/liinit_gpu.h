@@ -361,8 +361,27 @@ int liinit_assess_evaluate(liinit_ctx* h, const liinit_assess_params* p, const d
 /* Per-query values of the last evaluation, in query order (query j is stored point j * stride): h, v (NaN for a sparse or degenerate
  * query) and the neighbour count. *n = queries; any output may be NULL; LIINIT_ERR_CAPACITY when cap < queries. */
 int liinit_assess_download(liinit_ctx* h, double* h_out, double* v_out, int* n_out, long long cap, long long* n);
-/* Test hook: the points the last evaluation placed, xyz [cap*3] in stored order. *n = their number; xyz may be NULL. */
+/* Test hook: the points the last evaluation placed, xyz [cap*3] in stored order. *n = their number; xyz may be NULL. After a
+ * liinit_assess_cloud they are the points that call placed. */
 int liinit_assess_download_placed(liinit_ctx* h, float* xyz, long long cap, long long* n);
+/* Where the map is blurred: every stored point is a query (p->query_stride must be 0 or 1), placed and cell-sorted once, its moments
+ * summed in batches of at most LIINIT_ASSESS_MAX_QUERIES stored points. Point i's h, v and neighbour count are bit-equal to query i / s
+ * of a liinit_assess_evaluate with stride s dividing i and the same extrinsic. Records are 8 floats,
+ * x y z entropy plane_variance neighbors points valid:
+ *   leaf == 0: one per stored point, in stored order: the placed point, (float) h, v and n, points = 1, valid = 1 or 0 (h, v NaN).
+ *   leaf > 0:  one per occupied cubic leaf of edge leaf (leaf = floor(w / leaf) per axis, keyed over the placed bounding box like the
+ *              cells), in ascending key. fp64 sums of the leaf's per-point records, in stored order, stored as float: the centroid
+ *              and the mean neighbour count over all its points, mean h and v over its valid points (NaN when none is valid), the
+ *              point count and the valid count.
+ * rec8 == NULL asks for the number of records, *n (with totals == NULL too, nothing but the count is computed). *n is always set;
+ * cap_records < *n returns LIINIT_ERR_CAPACITY and writes neither rec8 nor totals. totals (may be NULL): the full-resolution counts,
+ * MME and MPV over every stored point (queries = points, stride 1). Records reach the host in chunks through the staging buffer;
+ * synchronises. Leaves the map, the staged cloud, the resident scan, the ICP state and the last evaluation's per-query values
+ * (liinit_assess_download) untouched. Errors as liinit_assess_evaluate, and LIINIT_ERR_INVALID for query_stride other than 0 or 1 or a
+ * negative or non-finite leaf; LIINIT_ERR_CAPACITY for a leaf so small that a placed point lies 2^30 leaves or more from the origin
+ * or the cloud spans more leaves than a 63-bit key holds. No device memory beyond liinit_assess_reserve's. */
+int liinit_assess_cloud(liinit_ctx* h, const liinit_assess_params* p, const double R_LI[9], const double T_LI[3], double leaf, float* rec8,
+                        long long cap_records, long long* n, liinit_assess_result* totals);
 
 #ifdef __cplusplus
 }

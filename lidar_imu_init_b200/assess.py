@@ -6,6 +6,9 @@ The sweep scores 14 candidates: the run as it went (each scan with its own extri
 rotated by +-DTHETA_DEG about each IMU axis (R = Exp(+-dtheta e_a) R_final) and shifted by +-DT_M along it. An axis whose two
 perturbations both score a higher MME than the final extrinsic is reported `constrained`, any other `flat`: the recording did not pin
 that axis down as far as this measure can tell. This is a report, not a verdict on the calibration.
+
+write_cloud shows where the as-run map is blurred: every stored point scored (LiInitGpu.assess_cloud), thinned to leaves on the device,
+as a PCD that a viewer colours by entropy.
 """
 from __future__ import annotations
 
@@ -19,6 +22,7 @@ RADIUS = 0.3            # neighbourhood radius [m]
 MIN_NEIGHBORS = 10
 MAX_POINTS = 30_000_000
 MAX_SCANS = 1 << 16
+CLOUD_LEAF = 0.1        # leaf edge of the assessment cloud [m]; 0: one record per stored point
 AXES = ("x", "y", "z")
 NOTHING = "nothing to assess: no LIO scan was stored (LI-Init did not trigger, or the run ended at the hand-over)\n"
 
@@ -88,6 +92,17 @@ class Assessment:
     def write(self, path: str):
         with open(path, "w") as f:
             f.write(self.report())
+
+    def write_cloud(self, path: str, leaf: float = CLOUD_LEAF):
+        """The per-point (leaf 0) or per-leaf entropy and plane variance of the as-run map, the map the run built, as a binary PCD
+        (pcd.write_assess). Returns (number of records, totals over every stored point), or None, writing nothing, when no scan was
+        stored."""
+        from . import pcd
+        if self.final is None:
+            return None
+        rec, tot = self.g.assess_cloud(radius=self.radius, min_neighbors=self.min_neighbors, leaf=leaf, as_run=True)
+        pcd.write_assess(path, rec)
+        return len(rec), tot
 
 
 def report_text(info: dict, radius: float, min_neighbors: int, sweep: list, dtheta_deg=DTHETA_DEG, dt=DT_M) -> str:

@@ -88,7 +88,7 @@ SYMBOLS = [
     "liinit_get_stream", "liinit_map_build_device", "liinit_map_add_points_device", "liinit_scan_upload_device", "liinit_raw_upload_device",
     "liinit_map_nearest_search_device", "liinit_cloud_download_device", "liinit_map_download_device",
     "liinit_assess_reserve", "liinit_assess_append", "liinit_assess_info", "liinit_assess_evaluate", "liinit_assess_download",
-    "liinit_assess_download_placed",
+    "liinit_assess_download_placed", "liinit_assess_cloud",
 ]
 
 
@@ -178,7 +178,9 @@ def set_assess_argtypes(L):
     L.liinit_assess_evaluate.argtypes = [vp, C.POINTER(AssessParams), vp, vp, C.POINTER(AssessResult)]
     L.liinit_assess_download.argtypes = [vp, vp, vp, vp, C.c_longlong, C.POINTER(C.c_longlong)]
     L.liinit_assess_download_placed.argtypes = [vp, vp, C.c_longlong, C.POINTER(C.c_longlong)]
-    for s in ("reserve", "append", "info", "evaluate", "download", "download_placed"):
+    L.liinit_assess_cloud.argtypes = [vp, C.POINTER(AssessParams), vp, vp, C.c_double, vp, C.c_longlong, C.POINTER(C.c_longlong),
+                                      C.POINTER(AssessResult)]
+    for s in ("reserve", "append", "info", "evaluate", "download", "download_placed", "cloud"):
         getattr(L, "liinit_assess_" + s).restype = C.c_int
 
 
@@ -670,6 +672,21 @@ class LiInitGpu:
         out = np.zeros((m.value, 3), np.float32)
         self._ck(self.L.liinit_assess_download_placed(self.h, _ptr(out), m.value, C.byref(m)))
         return out
+
+    def assess_cloud(self, R_LI=None, T_LI=None, radius: float = 0.3, min_neighbors: int = 10, leaf: float = 0.1, as_run: bool = False):
+        """Every stored point scored with the candidate extrinsic (as_run: each scan's own), as [n, 8] float32 records
+        x y z entropy plane_variance neighbors points valid: one per stored point (leaf 0) or per occupied leaf of edge `leaf` [m].
+        Returns (records, totals), totals the liinit_assess_result fields over every stored point. Leaves the last evaluation's
+        per-query values (assess_download) as they are."""
+        P = AssessParams(float(radius), int(min_neighbors), 1, int(bool(as_run)), 0)
+        R = None if R_LI is None else np.ascontiguousarray(R_LI, np.float64).reshape(9)
+        T = None if T_LI is None else np.ascontiguousarray(T_LI, np.float64).reshape(3)
+        n = C.c_longlong(0)
+        self._ck(self.L.liinit_assess_cloud(self.h, C.byref(P), _ptr(R), _ptr(T), float(leaf), None, 0, C.byref(n), None))
+        rec = np.zeros((n.value, 8), np.float32)
+        out = AssessResult()
+        self._ck(self.L.liinit_assess_cloud(self.h, C.byref(P), _ptr(R), _ptr(T), float(leaf), _ptr(rec), n.value, C.byref(n), C.byref(out)))
+        return rec[:n.value], {k: getattr(out, k) for k, _ in AssessResult._fields_}
 
     def knn_index(self) -> int:
         """1 = LIINIT_KNN_BRICKS (lockstep groups over whole bricks), 2 = LIINIT_KNN_CELLS (cell directory, thread per point)."""

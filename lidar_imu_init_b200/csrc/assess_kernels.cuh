@@ -6,6 +6,8 @@
 // The covariance of that neighbourhood gives the point's entropy h = 1/2 ln det(2 pi e Sigma) and plane variance v = lambda_min(Sigma).
 // Every query's value is a function of the stored data alone, and the totals are summed in query order by one block, so the results
 // are bit-identical from call to call and do not depend on the launch shape or the number of SMs.
+// A cloud (liinit_assess_cloud) takes every stored point as a query, in batches of consecutive stored indices over one placement and
+// sort, and turns the per-point values into 8-float records, one per point or, summed in stored order, one per occupied cubic leaf.
 #pragma once
 #include "common.cuh"
 #include "sort_kernels.cuh"
@@ -125,13 +127,18 @@ __global__ void k_as_gather(const float4* __restrict__ world, const unsigned lon
     skey[p] = key[i];
 }
 
+// stored point i is a query of the pass: every stride-th point with index in [qa, qb) (an evaluation: [0, n); a cloud: one batch)
+__device__ __forceinline__ int li_as_is_query(int i, int stride, int qa, int qb) {
+    return i % stride == 0 && i >= qa && i < qb ? 1 : 0;
+}
+
 // cell table and query list, step 1 (blockDim.x == LI_FR_TILE): per block the number of cell starts (tc) and of queries (tq); block 0
 // zeroes tc[gridDim.x] and tq[gridDim.x], which the exclusive scans turn into the totals
-__global__ void k_as_mark(const unsigned long long* __restrict__ skey, const float4* __restrict__ sorted, int n, int stride, int* __restrict__ tc,
-                          int* __restrict__ tq) {
+__global__ void k_as_mark(const unsigned long long* __restrict__ skey, const float4* __restrict__ sorted, int n, int stride, int qa, int qb,
+                          int* __restrict__ tc, int* __restrict__ tq) {
     const int p = blockIdx.x * blockDim.x + threadIdx.x;
     const int fc = p < n && (p == 0 || skey[p] != skey[p - 1]) ? 1 : 0;
-    const int fq = p < n && __float_as_int(sorted[p].w) % stride == 0 ? 1 : 0;
+    const int fq = p < n ? li_as_is_query(__float_as_int(sorted[p].w), stride, qa, qb) : 0;
     int t1, t2;
     li_block_excl_scan(fc, &t1);
     __syncthreads();   // li_block_excl_scan's shared words are reused by the second scan
@@ -145,12 +152,12 @@ __global__ void k_as_mark(const unsigned long long* __restrict__ skey, const flo
 
 // step 2 (tc, tq: exclusive per-block offsets): cell c starts at sorted position cell_start[c], has key cell_key[c] and its queries are
 // qlist[cell_q0[c] .. cell_q0[c + 1]); the sentinels cell_start[ncells] = n and cell_q0[ncells] = queries close the tables
-__global__ void k_as_index(const unsigned long long* __restrict__ skey, const float4* __restrict__ sorted, int n, int stride, const int* __restrict__ tc,
-                           const int* __restrict__ tq, int* __restrict__ cell_start, unsigned long long* __restrict__ cell_key, int* __restrict__ cell_q0,
-                           int* __restrict__ qlist) {
+__global__ void k_as_index(const unsigned long long* __restrict__ skey, const float4* __restrict__ sorted, int n, int stride, int qa, int qb,
+                           const int* __restrict__ tc, const int* __restrict__ tq, int* __restrict__ cell_start, unsigned long long* __restrict__ cell_key,
+                           int* __restrict__ cell_q0, int* __restrict__ qlist) {
     const int p = blockIdx.x * blockDim.x + threadIdx.x;
     const int fc = p < n && (p == 0 || skey[p] != skey[p - 1]) ? 1 : 0;
-    const int fq = p < n && __float_as_int(sorted[p].w) % stride == 0 ? 1 : 0;
+    const int fq = p < n ? li_as_is_query(__float_as_int(sorted[p].w), stride, qa, qb) : 0;
     int t;
     const int c = tc[blockIdx.x] + li_block_excl_scan(fc, &t);
     __syncthreads();
@@ -344,4 +351,78 @@ __global__ void k_as_reduce(const int* __restrict__ qn, const double* __restrict
         out->sparse = s_c[1][0];
         out->degenerate = s_c[2][0];
     }
+}
+
+// ---- the per-point cloud (liinit_assess_cloud, DESIGN.md section 4d) ----
+// Every stored point is a query: the moments above run in batches of consecutive stored indices and write the per-point n, h, v by stored
+// index. A record is 8 floats: x y z entropy plane_variance neighbors points valid.
+
+// one record per stored point a + j, j < m, from the placed point and its per-point values (valid: h is not NaN)
+__global__ void k_ac_point_rec(const float4* __restrict__ world, const double* __restrict__ qh, const double* __restrict__ qv,
+                               const int* __restrict__ qn, int a, int m, float4* __restrict__ rec) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= m) return;
+    const int i = a + j;
+    const float4 w = world[i];
+    const double h = qh[i];
+    rec[2 * j] = make_float4(w.x, w.y, w.z, (float)h);
+    rec[2 * j + 1] = make_float4((float)qv[i], (float)qn[i], 1.f, h == h ? 1.f : 0.f);
+}
+
+// the per-point values as they go into a record (h, v, neighbours, valid), for the leaf sums
+__global__ void k_ac_point_pack(const double* __restrict__ qh, const double* __restrict__ qv, const int* __restrict__ qn, int n,
+                                float4* __restrict__ hvn) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const double h = qh[i];
+    hvn[i] = make_float4((float)h, (float)qv[i], (float)qn[i], h == h ? 1.f : 0.f);
+}
+
+// leaf table, step 1 (blockDim.x == LI_FR_TILE): per block the number of leaf starts in the sorted order perm; block 0 zeroes tl[gridDim.x]
+__global__ void k_ac_leaf_mark(const unsigned long long* __restrict__ key, const unsigned* __restrict__ perm, int n, int* __restrict__ tl) {
+    const int p = blockIdx.x * blockDim.x + threadIdx.x;
+    const int f = p < n && (p == 0 || key[perm[p]] != key[perm[p - 1]]) ? 1 : 0;
+    int t;
+    li_block_excl_scan(f, &t);
+    if (threadIdx.x == 0) {
+        tl[blockIdx.x] = t;
+        if (blockIdx.x == 0) tl[gridDim.x] = 0;
+    }
+}
+
+// step 2 (tl: exclusive per-block offsets): leaf c covers sorted positions leaf_start[c] .. leaf_start[c + 1]; the sentinel
+// leaf_start[leaves] = n closes the table
+__global__ void k_ac_leaf_index(const unsigned long long* __restrict__ key, const unsigned* __restrict__ perm, int n, const int* __restrict__ tl,
+                                int* __restrict__ leaf_start) {
+    const int p = blockIdx.x * blockDim.x + threadIdx.x;
+    const int f = p < n && (p == 0 || key[perm[p]] != key[perm[p - 1]]) ? 1 : 0;
+    int t;
+    const int c = tl[blockIdx.x] + li_block_excl_scan(f, &t);
+    if (f) leaf_start[c] = p;
+    if (p == 0) leaf_start[tl[gridDim.x]] = n;
+}
+
+// one record per leaf c0 + j, j < m: one thread sums the leaf's points in stored order (the sort is stable over the identity permutation)
+// in fp64; centroid and mean neighbour count over all of them, mean h and v over the valid ones (NaN when there is none)
+__global__ void k_ac_leaf_rec(const float4* __restrict__ world, const float4* __restrict__ hvn, const unsigned* __restrict__ perm,
+                              const int* __restrict__ leaf_start, int c0, int m, float4* __restrict__ rec) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= m) return;
+    const int b = leaf_start[c0 + j], e = leaf_start[c0 + j + 1];
+    double sx = 0.0, sy = 0.0, sz = 0.0, sh = 0.0, sv = 0.0, sn = 0.0;
+    int nv = 0;
+    for (int p = b; p < e; p++) {
+        const unsigned i = perm[p];
+        const float4 w = world[i], a = hvn[i];
+        sx += w.x; sy += w.y; sz += w.z;
+        sn += a.z;
+        if (a.w != 0.f) {
+            sh += a.x; sv += a.y;
+            nv++;
+        }
+    }
+    const double np = (double)(e - b);
+    const float nan = __int_as_float(0x7fc00000);
+    rec[2 * j] = make_float4((float)(sx / np), (float)(sy / np), (float)(sz / np), nv ? (float)(sh / nv) : nan);
+    rec[2 * j + 1] = make_float4(nv ? (float)(sv / nv) : nan, (float)(sn / np), (float)(e - b), (float)nv);
 }

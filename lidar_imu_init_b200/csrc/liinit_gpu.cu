@@ -216,7 +216,7 @@ struct Ctx {
         float4* sorted = nullptr;  // placed points in cell order, w = stored index
         unsigned long long* key = nullptr;
         unsigned long long* skey = nullptr;
-        unsigned* k[2] = {nullptr, nullptr};
+        unsigned* k[2] = {nullptr, nullptr};   // one allocation of 2 N words: k[1] = k[0] + N
         unsigned* v[2] = {nullptr, nullptr};
         int* hist = nullptr;
         int* tc = nullptr;   // per-block counts: cell starts, queries, tasks
@@ -786,7 +786,7 @@ const FrameSub* frame_lookup(Ctx* c, long long handle, int* slot) {
 void assess_free(Ctx* c) {
     Ctx::Assess& A = c->A;
     cudaFree(A.pts); cudaFree(A.poses); cudaFree(A.world); cudaFree(A.sorted); cudaFree(A.key); cudaFree(A.skey);
-    cudaFree(A.k[0]); cudaFree(A.k[1]); cudaFree(A.v[0]); cudaFree(A.v[1]); cudaFree(A.hist); cudaFree(A.tc); cudaFree(A.tq); cudaFree(A.tt);
+    cudaFree(A.k[0]); cudaFree(A.v[0]); cudaFree(A.v[1]); cudaFree(A.hist); cudaFree(A.tc); cudaFree(A.tq); cudaFree(A.tt);
     cudaFree(A.cell_start); cudaFree(A.cell_key); cudaFree(A.cell_q0); cudaFree(A.qlist); cudaFree(A.tasks); cudaFree(A.qn); cudaFree(A.qh);
     cudaFree(A.qv); cudaFree(A.box); cudaFree(A.tot); cudaFree(A.ticket);
     A = Ctx::Assess{};
@@ -2270,44 +2270,51 @@ int assess_sort_pass(Ctx* c, int& cur, int n, int shift) {
     return LIINIT_OK;
 }
 
-int assess_evaluate(Ctx* c, const liinit_assess_params* prm, const double* R_LI, const double* T_LI, liinit_assess_result* out) {
-    Ctx::Assess& A = c->A;
+// the checks liinit_assess_evaluate and liinit_assess_cloud share; a cloud takes every stored point as a query (stride 0 or 1)
+int assess_check_params(Ctx* c, const liinit_assess_params* prm, const double* R_LI, const double* T_LI, bool cloud) {
     const double r = prm->radius;
     if (!std::isfinite(r) || !(r > 0.0)) return fail(c, LIINIT_ERR_INVALID, "radius must be positive and finite");
     if (prm->min_neighbors < 4) return fail(c, LIINIT_ERR_INVALID, "min_neighbors must be at least 4");
-    if (prm->query_stride < 0) return fail(c, LIINIT_ERR_INVALID, "query_stride must be >= 0 (0: automatic)");
+    if (!cloud && prm->query_stride < 0) return fail(c, LIINIT_ERR_INVALID, "query_stride must be >= 0 (0: automatic)");
+    if (cloud && prm->query_stride != 0 && prm->query_stride != 1)
+        return fail(c, LIINIT_ERR_INVALID, "a cloud takes every stored point as a query: query_stride must be 0 or 1");
     if (!prm->as_run && (!R_LI || !T_LI)) return fail(c, LIINIT_ERR_INVALID, "a candidate extrinsic needs R_LI and T_LI (or as_run)");
     if (!prm->as_run)
         for (int k = 0; k < 12; k++)
             if (!std::isfinite(k < 9 ? R_LI[k] : T_LI[k - 9])) return fail(c, LIINIT_ERR_INVALID, "R_LI / T_LI must be finite");
-    if (A.n == 0) return fail(c, LIINIT_ERR_INVALID, "the assessment store is empty (liinit_assess_append)");
+    return LIINIT_OK;
+}
+
+// k_as_place into A.world, then the grid of cubic cells of edge `edge` over the placed bounding box (one synchronisation); leaf: the
+// cells are the leaves of a cloud
+int assess_place(Ctx* c, int as_run, const PoseD& cand, double edge, bool leaf, AsGrid& G) {
+    Ctx::Assess& A = c->A;
     const int n = (int)A.n;
-    const long long s = prm->query_stride > 0 ? prm->query_stride : (A.n + LIINIT_ASSESS_MAX_QUERIES - 1) / LIINIT_ASSESS_MAX_QUERIES;
-    const long long nq = (A.n + s - 1) / s;
-    if (nq > LIINIT_ASSESS_MAX_QUERIES)
-        return fail(c, LIINIT_ERR_CAPACITY, "query_stride gives " + std::to_string(nq) + " queries, more than LIINIT_ASSESS_MAX_QUERIES");
-    PoseD cand{};
-    if (!prm->as_run) {
-        memcpy(cand.RLI, R_LI, 72);
-        memcpy(cand.TLI, T_LI, 24);
-    }
-    const double edge = r * (1.0 + ldexp(1.0, -20));
     int box[8] = {0x7fffffff, 0x7fffffff, 0x7fffffff, -0x7fffffff - 1, -0x7fffffff - 1, -0x7fffffff - 1, 0, 0};
     CU(cudaMemcpyAsync(A.box, box, sizeof(box), cudaMemcpyHostToDevice, c->stream));
-    k_as_place<<<nblk(n, 256), 256, 0, c->stream>>>(A.pts, A.poses, n, prm->as_run ? 1 : 0, cand, edge, A.world, A.box);
+    k_as_place<<<nblk(n, 256), 256, 0, c->stream>>>(A.pts, A.poses, n, as_run, cand, edge, A.world, A.box);
     c->launches++;
     CU(cudaGetLastError());
     CU(cudaMemcpyAsync(box, A.box, sizeof(box), cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
-    if (box[6]) return fail(c, LIINIT_ERR_CAPACITY, "a placed point is not finite or lies 2^30 cells or more from the origin");
-    AsGrid G;
+    if (box[6])
+        return fail(c, LIINIT_ERR_CAPACITY, std::string("a placed point is not finite or lies 2^30 ") + (leaf ? "leaves" : "cells") + " or more from the origin");
     G.edge = edge;
     for (int a = 0; a < 3; a++) {
         G.lo[a] = box[a];
         G.ext[a] = (long long)box[3 + a] - box[a] + 1;
     }
     if ((double)G.ext[0] * (double)G.ext[1] * (double)G.ext[2] > 9.0e18)
-        return fail(c, LIINIT_ERR_CAPACITY, "the placed cloud spans more cells than a 63-bit cell key holds");
+        return fail(c, LIINIT_ERR_CAPACITY, leaf ? "the placed cloud spans more leaves than a 63-bit leaf key holds"
+                                                 : "the placed cloud spans more cells than a 63-bit cell key holds");
+    return LIINIT_OK;
+}
+
+// keys of A.world on the grid G (A.key) and the stable radix sort of the identity permutation by them: the sorted stored indices end in
+// A.v[cur]
+int assess_sort(Ctx* c, const AsGrid& G, int& cur) {
+    Ctx::Assess& A = c->A;
+    const int n = (int)A.n;
     const unsigned long long cells = (unsigned long long)G.ext[0] * (unsigned long long)G.ext[1] * (unsigned long long)G.ext[2];
     int bits = 0;
     while (bits < 64 && ((cells - 1) >> bits)) bits++;
@@ -2315,7 +2322,7 @@ int assess_evaluate(Ctx* c, const liinit_assess_params* prm, const double* R_LI,
     c->launches++;
     CU(cudaGetLastError());
     // stable sort by cell key: the low word's digits, then (keys wider than 32 bits) the high word's; only the digits the box needs
-    int cur = 0;
+    cur = 0;
     for (int sh = 0; sh < bits && sh < 32; sh += 8) {
         const int rc = assess_sort_pass(c, cur, n, sh);
         if (rc) return rc;
@@ -2328,14 +2335,47 @@ int assess_evaluate(Ctx* c, const liinit_assess_params* prm, const double* R_LI,
             if (rc) return rc;
         }
     }
+    return LIINIT_OK;
+}
+
+// the candidate's extrinsic (unused with as_run)
+PoseD assess_candidate(const liinit_assess_params* prm, const double* R_LI, const double* T_LI) {
+    PoseD cand{};
+    if (!prm->as_run) {
+        memcpy(cand.RLI, R_LI, 72);
+        memcpy(cand.TLI, T_LI, 24);
+    }
+    return cand;
+}
+
+// the cell edge of a radius: r (1 + 2^-20), see li_as_cell
+double assess_edge(double r) { return r * (1.0 + ldexp(1.0, -20)); }
+
+int assess_evaluate(Ctx* c, const liinit_assess_params* prm, const double* R_LI, const double* T_LI, liinit_assess_result* out) {
+    Ctx::Assess& A = c->A;
+    const double r = prm->radius;
+    int rc = assess_check_params(c, prm, R_LI, T_LI, false);
+    if (rc) return rc;
+    if (A.n == 0) return fail(c, LIINIT_ERR_INVALID, "the assessment store is empty (liinit_assess_append)");
+    const int n = (int)A.n;
+    const long long s = prm->query_stride > 0 ? prm->query_stride : (A.n + LIINIT_ASSESS_MAX_QUERIES - 1) / LIINIT_ASSESS_MAX_QUERIES;
+    const long long nq = (A.n + s - 1) / s;
+    if (nq > LIINIT_ASSESS_MAX_QUERIES)
+        return fail(c, LIINIT_ERR_CAPACITY, "query_stride gives " + std::to_string(nq) + " queries, more than LIINIT_ASSESS_MAX_QUERIES");
+    AsGrid G;
+    rc = assess_place(c, prm->as_run ? 1 : 0, assess_candidate(prm, R_LI, T_LI), assess_edge(r), false, G);
+    if (rc) return rc;
+    int cur;
+    rc = assess_sort(c, G, cur);
+    if (rc) return rc;
     k_as_gather<<<nblk(n, 256), 256, 0, c->stream>>>(A.world, A.key, A.v[cur], n, A.sorted, A.skey);
     c->launches++;
     const int nb = nblk(n, LI_FR_TILE);
     const int qs = (int)s;
-    k_as_mark<<<nb, LI_FR_TILE, 0, c->stream>>>(A.skey, A.sorted, n, qs, A.tc, A.tq);
+    k_as_mark<<<nb, LI_FR_TILE, 0, c->stream>>>(A.skey, A.sorted, n, qs, 0, n, A.tc, A.tq);
     k_rs_scan<<<1, 1024, 0, c->stream>>>(nb + 1, A.tc);
     k_rs_scan<<<1, 1024, 0, c->stream>>>(nb + 1, A.tq);
-    k_as_index<<<nb, LI_FR_TILE, 0, c->stream>>>(A.skey, A.sorted, n, qs, A.tc, A.tq, A.cell_start, A.cell_key, A.cell_q0, A.qlist);
+    k_as_index<<<nb, LI_FR_TILE, 0, c->stream>>>(A.skey, A.sorted, n, qs, 0, n, A.tc, A.tq, A.cell_start, A.cell_key, A.cell_q0, A.qlist);
     // (there are at most n cells: nb blocks cover them)
     k_as_task_count<<<nb, LI_FR_TILE, 0, c->stream>>>(A.cell_q0, A.tc + nb, A.tt);
     k_rs_scan<<<1, 1024, 0, c->stream>>>(nb + 1, A.tt);
@@ -2365,6 +2405,139 @@ int assess_evaluate(Ctx* c, const liinit_assess_params* prm, const double* R_LI,
     return LIINIT_OK;
 }
 
+// stored points per moments batch of a cloud: the per-query buffers liinit_assess_reserve sizes for LIINIT_ASSESS_MAX_QUERIES queries
+// hold one batch (a smaller value only splits the work more finely; the CPU tests build one)
+#ifndef LI_AS_CLOUD_BATCH
+#define LI_AS_CLOUD_BATCH LIINIT_ASSESS_MAX_QUERIES
+#endif
+static_assert(LI_AS_CLOUD_BATCH > 0 && LI_AS_CLOUD_BATCH <= LIINIT_ASSESS_MAX_QUERIES, "a cloud batch must fit the per-query buffers");
+
+// leaves of A.world on the grid L: the stored indices in leaf order in A.v[cur] (stored order inside a leaf), leaf c at sorted
+// positions A.cell_start[c] .. A.cell_start[c + 1]; *leaves = their number (one synchronisation)
+int assess_leaf_table(Ctx* c, const AsGrid& L, int& cur, long long& leaves) {
+    Ctx::Assess& A = c->A;
+    const int n = (int)A.n;
+    int rc = assess_sort(c, L, cur);
+    if (rc) return rc;
+    const int nb = nblk(n, LI_FR_TILE);
+    k_ac_leaf_mark<<<nb, LI_FR_TILE, 0, c->stream>>>(A.key, A.v[cur], n, A.tc);
+    k_rs_scan<<<1, 1024, 0, c->stream>>>(nb + 1, A.tc);
+    k_ac_leaf_index<<<nb, LI_FR_TILE, 0, c->stream>>>(A.key, A.v[cur], n, A.tc, A.cell_start);
+    c->launches += 3;
+    CU(cudaGetLastError());
+    int m = 0;
+    CU(cudaMemcpyAsync(&m, A.tc + nb, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    leaves = m;
+    return LIINIT_OK;
+}
+
+int assess_cloud(Ctx* c, const liinit_assess_params* prm, const double* R_LI, const double* T_LI, double leaf, float* rec8, long long cap,
+                 long long* n_out, liinit_assess_result* out) {
+    Ctx::Assess& A = c->A;
+    int rc = assess_check_params(c, prm, R_LI, T_LI, true);
+    if (rc) return rc;
+    if (!std::isfinite(leaf) || leaf < 0.0) return fail(c, LIINIT_ERR_INVALID, "leaf must be >= 0 and finite (0: one record per stored point)");
+    if (A.n == 0) return fail(c, LIINIT_ERR_INVALID, "the assessment store is empty (liinit_assess_append)");
+    const int n = (int)A.n, as_run = prm->as_run ? 1 : 0, min_nb = prm->min_neighbors;
+    const double r = prm->radius;
+    const PoseD cand = assess_candidate(prm, R_LI, T_LI);
+    AsGrid L{};
+    int cur = 0;
+    long long records = n;
+    if (leaf == 0.0) {
+        *n_out = records;
+        if (rec8 && cap < records) return fail(c, LIINIT_ERR_CAPACITY, "cap_records is smaller than the number of records");
+        if (!rec8 && !out) return LIINIT_OK;
+    } else {
+        // the leaf grid first: a leaf too small for the cloud is refused before the moments run
+        rc = assess_place(c, as_run, cand, leaf, true, L);
+        if (rc) return rc;
+        if (!rec8 && !out) {
+            rc = assess_leaf_table(c, L, cur, records);
+            if (rc) return rc;
+            *n_out = records;
+            return LIINIT_OK;
+        }
+    }
+    // place and cell-sort once (the placement is the one above: same points, poses and extrinsics)
+    AsGrid G;
+    rc = assess_place(c, as_run, cand, assess_edge(r), false, G);
+    if (rc) return rc;
+    rc = assess_sort(c, G, cur);
+    if (rc) return rc;
+    k_as_gather<<<nblk(n, 256), 256, 0, c->stream>>>(A.world, A.key, A.v[cur], n, A.sorted, A.skey);
+    c->launches++;
+    CU(cudaGetLastError());
+    // per-point n, h, v by stored index, in the sort buffers the gather has freed: A.v[0] (n ints), A.key and the A.k pair (one
+    // allocation) as n doubles each. A.qn / A.qh / A.qv keep the last evaluation's values.
+    int* pn = reinterpret_cast<int*>(A.v[0]);
+    double* ph = reinterpret_cast<double*>(A.key);
+    double* pv = reinterpret_cast<double*>(A.k[0]);
+    const int nb = nblk(n, LI_FR_TILE);
+    for (int a = 0; a < n; a += LI_AS_CLOUD_BATCH) {
+        const int b = n - a > LI_AS_CLOUD_BATCH ? a + LI_AS_CLOUD_BATCH : n;   // the queries of this batch: stored points [a, b)
+        k_as_mark<<<nb, LI_FR_TILE, 0, c->stream>>>(A.skey, A.sorted, n, 1, a, b, A.tc, A.tq);
+        k_rs_scan<<<1, 1024, 0, c->stream>>>(nb + 1, A.tc);
+        k_rs_scan<<<1, 1024, 0, c->stream>>>(nb + 1, A.tq);
+        k_as_index<<<nb, LI_FR_TILE, 0, c->stream>>>(A.skey, A.sorted, n, 1, a, b, A.tc, A.tq, A.cell_start, A.cell_key, A.cell_q0, A.qlist);
+        k_as_task_count<<<nb, LI_FR_TILE, 0, c->stream>>>(A.cell_q0, A.tc + nb, A.tt);
+        k_rs_scan<<<1, 1024, 0, c->stream>>>(nb + 1, A.tt);
+        k_as_task_emit<<<nb, LI_FR_TILE, 0, c->stream>>>(A.cell_q0, A.tc + nb, A.tt, A.tasks);
+        c->launches += 7;
+        CU(cudaGetLastError());
+        CU(cudaMemsetAsync(A.ticket, 0, sizeof(unsigned), c->stream));
+        k_as_moments<<<c->num_sms * 8, LI_AS_BLOCK, 0, c->stream>>>(A.sorted, A.cell_start, A.cell_key, A.tc + nb, A.qlist, A.tasks, A.tt + nb,
+                                                                    A.ticket, G, r * r, 1, min_nb, pn, ph, pv);
+        c->launches++;
+        CU(cudaGetLastError());
+    }
+    k_as_reduce<<<1, 1024, 0, c->stream>>>(pn, ph, pv, n, min_nb, A.tot);
+    c->launches++;
+    CU(cudaGetLastError());
+    AsTotals T;
+    CU(cudaMemcpyAsync(&T, A.tot, sizeof(T), cudaMemcpyDeviceToHost, c->stream));
+    if (leaf > 0.0) {
+        // the record values of every point into A.sorted (free now), then the leaf sort (it reuses A.key, A.k, A.v)
+        k_ac_point_pack<<<nblk(n, 256), 256, 0, c->stream>>>(ph, pv, pn, n, A.sorted);
+        c->launches++;
+        CU(cudaGetLastError());
+        rc = assess_leaf_table(c, L, cur, records);
+        if (rc) return rc;
+        *n_out = records;
+        if (rec8 && cap < records) return fail(c, LIINIT_ERR_CAPACITY, "cap_records is smaller than the number of records");
+    } else {
+        CU(cudaStreamSynchronize(c->stream));
+    }
+    if (out) {
+        out->points = A.n;
+        out->queries = A.n;
+        out->stride = 1;
+        out->scans = A.scans;
+        out->valid = T.valid;
+        out->sparse = T.sparse;
+        out->degenerate = T.degenerate;
+        out->mme = T.valid ? T.sum_h / (double)T.valid : NAN;
+        out->mpv = T.valid ? T.sum_v / (double)T.valid : NAN;
+    }
+    if (!rec8) return LIINIT_OK;
+    // the records reach the host in chunks through the strided staging buffer (free once a cloud is repacked)
+    const long long chunk = (long long)(c->stage_raw_floats / 8);
+    float4* stage = reinterpret_cast<float4*>(c->d_stage_raw);
+    for (long long a = 0; a < records; a += chunk) {
+        const int m = (int)(records - a < chunk ? records - a : chunk);
+        if (leaf > 0.0)
+            k_ac_leaf_rec<<<nblk(m, 256), 256, 0, c->stream>>>(A.world, A.sorted, A.v[cur], A.cell_start, (int)a, m, stage);
+        else
+            k_ac_point_rec<<<nblk(m, 256), 256, 0, c->stream>>>(A.world, ph, pv, pn, (int)a, m, stage);
+        c->launches++;
+        CU(cudaGetLastError());
+        CU(cudaMemcpyAsync(rec8 + 8 * (size_t)a, stage, (size_t)m * 8 * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+    }
+    CU(cudaStreamSynchronize(c->stream));
+    return LIINIT_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -2383,14 +2556,15 @@ int liinit_assess_reserve(liinit_ctx* h, long long max_points, int max_scans) {
     const size_t NB = N / LI_FR_TILE + 2;
     bool ok = cudaMalloc(&A.pts, N * sizeof(float4)) == cudaSuccess && cudaMalloc(&A.poses, (size_t)max_scans * sizeof(PoseD)) == cudaSuccess &&
               cudaMalloc(&A.world, N * sizeof(float4)) == cudaSuccess && cudaMalloc(&A.sorted, N * sizeof(float4)) == cudaSuccess &&
-              cudaMalloc(&A.key, N * 8) == cudaSuccess && cudaMalloc(&A.skey, N * 8) == cudaSuccess && cudaMalloc(&A.k[0], N * 4) == cudaSuccess &&
-              cudaMalloc(&A.k[1], N * 4) == cudaSuccess && cudaMalloc(&A.v[0], N * 4) == cudaSuccess && cudaMalloc(&A.v[1], N * 4) == cudaSuccess &&
+              cudaMalloc(&A.key, N * 8) == cudaSuccess && cudaMalloc(&A.skey, N * 8) == cudaSuccess && cudaMalloc(&A.k[0], N * 8) == cudaSuccess &&
+              cudaMalloc(&A.v[0], N * 4) == cudaSuccess && cudaMalloc(&A.v[1], N * 4) == cudaSuccess &&
               cudaMalloc(&A.hist, (N / RS_TILE + 2) * 256 * 4) == cudaSuccess && cudaMalloc(&A.tc, NB * 4) == cudaSuccess &&
               cudaMalloc(&A.tq, NB * 4) == cudaSuccess && cudaMalloc(&A.tt, NB * 4) == cudaSuccess && cudaMalloc(&A.cell_start, (N + 1) * 4) == cudaSuccess &&
               cudaMalloc(&A.cell_key, N * 8) == cudaSuccess && cudaMalloc(&A.cell_q0, (N + 1) * 4) == cudaSuccess && cudaMalloc(&A.qlist, Q * 4) == cudaSuccess &&
               cudaMalloc(&A.tasks, Q * sizeof(int4)) == cudaSuccess && cudaMalloc(&A.qn, Q * 4) == cudaSuccess && cudaMalloc(&A.qh, Q * 8) == cudaSuccess &&
               cudaMalloc(&A.qv, Q * 8) == cudaSuccess && cudaMalloc(&A.box, 8 * 4) == cudaSuccess && cudaMalloc(&A.tot, sizeof(AsTotals)) == cudaSuccess &&
               cudaMalloc(&A.ticket, sizeof(unsigned)) == cudaSuccess;
+    if (ok) A.k[1] = A.k[0] + N;   // one allocation: a cloud keeps n doubles in it (assess_cloud)
     if (!ok) {
         cudaGetLastError();
         assess_free(c);
@@ -2446,6 +2620,17 @@ int liinit_assess_evaluate(liinit_ctx* h, const liinit_assess_params* p, const d
     if (r) return r;
     CU(cudaSetDevice(c->device));
     return assess_evaluate(c, p, R_LI, T_LI, out);
+}
+
+int liinit_assess_cloud(liinit_ctx* h, const liinit_assess_params* p, const double R_LI[9], const double T_LI[3], double leaf, float* rec8,
+                        long long cap_records, long long* n, liinit_assess_result* totals) {
+    if (!h) return LIINIT_ERR_INVALID;
+    Ctx* c = &h->c;
+    if (!p || !n) return fail(c, LIINIT_ERR_INVALID, "null argument");
+    int r = assess_check(c);
+    if (r) return r;
+    CU(cudaSetDevice(c->device));
+    return assess_cloud(c, p, R_LI, T_LI, leaf, rec8, cap_records, n, totals);
 }
 
 int liinit_assess_download(liinit_ctx* h, double* h_out, double* v_out, int* n_out, long long cap, long long* n) {

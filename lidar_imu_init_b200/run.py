@@ -3,7 +3,8 @@
     python -m lidar_imu_init_b200.run --config avia.yaml --bag rec.bag [--out DIR] [--param name=value ...] [--device N]
                                       [--max-map-points N] [--record PATH [--record-format ros1|ros2]
                                       [--record-compression none|bz2] [--record-topics a,b,...]] [--debug-logs]
-                                      [--assess [--assess-radius R] [--assess-max-points N]]
+                                      [--assess] [--assess-cloud PATH [--assess-cloud-leaf L]] [--assess-radius R]
+                                      [--assess-max-points N]
 
 --bag is a ROS1 bag (v2.0), a rosbag2 directory (sqlite3 storage) or one of its .db3 files, told apart by the file's first bytes. The
 LiDAR topic carries livox_ros_driver/CustomMsg or livox_ros_driver2/CustomMsg (lidar_type 1) or sensor_msgs/PointCloud2 in a ROS1
@@ -20,6 +21,8 @@ directory for a ROS 2 input, or as --record-format says. --debug-logs writes LI-
 
 --assess stores the LIO scans on the device and, at the end of the run, scores the calibration by how sharp a map it builds: the mean
 map entropy and plane variance of the as-run, final and perturbed extrinsics, written to DIR/result/assessment.txt (assess).
+--assess-cloud PATH (with or without --assess) writes where the as-run map is blurred: the entropy and plane variance of every stored
+point, averaged over cubic leaves of --assess-cloud-leaf metres (0: every point), as a binary PCD.
 """
 from __future__ import annotations
 
@@ -59,6 +62,10 @@ def parse_args(argv=None):
                     "DIR/result/assessment.txt")
     ap.add_argument("--assess-radius", type=float, default=assessmod.RADIUS, metavar="R",
                     help=f"neighbourhood radius of the assessment [m] (default {assessmod.RADIUS:g})")
+    ap.add_argument("--assess-cloud", metavar="PATH", help="write the per-point map entropy and plane variance of the as-run map, "
+                    "thinned to leaves, as a binary PCD at PATH (stores the LIO scans like --assess)")
+    ap.add_argument("--assess-cloud-leaf", type=float, default=assessmod.CLOUD_LEAF, metavar="L",
+                    help=f"leaf edge of --assess-cloud [m] (default {assessmod.CLOUD_LEAF:g}; 0: one record per stored point)")
     ap.add_argument("--assess-max-points", type=int, default=assessmod.MAX_POINTS, metavar="N",
                     help=f"LIO points the assessment stores on the device (default {assessmod.MAX_POINTS}); later scans are skipped")
     return ap.parse_args(argv)
@@ -96,9 +103,12 @@ def main(argv=None, on_node=None) -> int:
     try:
         cfg = cfgmod.load(args.config, args.param)
         topics = record_topics(args)
-        if args.assess and not (args.assess_radius > 0 and args.assess_radius < float("inf")):
+        assessing = args.assess or args.assess_cloud is not None
+        if assessing and not (args.assess_radius > 0 and args.assess_radius < float("inf")):
             raise cfgmod.ConfigError(f"--assess-radius {args.assess_radius!r}: must be a positive number of metres")
-        if args.assess and args.assess_max_points < 1:
+        if args.assess_cloud is not None and not (args.assess_cloud_leaf >= 0 and args.assess_cloud_leaf < float("inf")):
+            raise cfgmod.ConfigError(f"--assess-cloud-leaf {args.assess_cloud_leaf!r}: must be zero or a positive number of metres")
+        if assessing and args.assess_max_points < 1:
             raise cfgmod.ConfigError(f"--assess-max-points {args.assess_max_points}: must be positive")
         with rosbag2.open_bag(args.bag) as bag:
             bag.check_topics(cfgmod.wanted_topics(cfg, bag.format))
@@ -111,7 +121,7 @@ def main(argv=None, on_node=None) -> int:
                 node.recorder = Recorder(writer, cfg, topics)
             if args.debug_logs:
                 node.open_debug_logs()
-            if args.assess:
+            if assessing:
                 node.assess = assessmod.Assessment(node.odom.g, args.assess_max_points, args.assess_radius)
             if on_node is not None:
                 on_node(node)
@@ -119,10 +129,18 @@ def main(argv=None, on_node=None) -> int:
             node.run(bag)
             wall = time.perf_counter() - t0
         node.close()
-        if node.assess is not None:
+        if args.assess:
             t0 = time.perf_counter()
             node.assess.write(os.path.join(args.out, "result", "assessment.txt"))
             log.info(f"assessment written to {os.path.join(args.out, 'result', 'assessment.txt')} in {time.perf_counter() - t0:.1f} s")
+        if args.assess_cloud is not None:
+            t0 = time.perf_counter()
+            got = node.assess.write_cloud(args.assess_cloud, args.assess_cloud_leaf)
+            if got is None:
+                log.warn(f"{args.assess_cloud} not written: {assessmod.NOTHING.strip()}")
+            else:
+                log.info(f"assessment cloud written to {args.assess_cloud}: {got[0]} records, full-resolution MME {got[1]['mme']:.6f} over "
+                         f"{got[1]['valid']} of {got[1]['points']} points, in {time.perf_counter() - t0:.1f} s")
         node.odom.g.close()
         log.info(f"{node.updates} updates in {wall:.1f} s; {node.odom.dropped_subframes} sub-frames dropped")
         return 0
