@@ -247,9 +247,9 @@ int liinit_scan_upload_device(liinit_ctx* h, const float* body_xyz, int stride_f
 /* liinit_raw_upload: repacked from the caller's memory; the PointType layout (stride >= 12, time_index 9) brings normals and intensity
  * along as the twin does. No synchronisation. */
 int liinit_raw_upload_device(liinit_ctx* h, const float* pts, int stride_floats, int time_index, int n);
-/* liinit_map_nearest_search: queries, out_xyz [n*5*3], out_d2 [n*5] and out_cnt [n] on the device (any output may be NULL). The count
- * and the PointType_CMP tie order (ikd_Tree.h:57-60, applied when both out_xyz and out_d2 are given) are computed on the device,
- * exactly as the twin computes them on the host. No synchronisation, any n. */
+/* liinit_map_nearest_search: queries, out_xyz [n*5*3], out_d2 [n*5] and out_cnt [n] on the device (any output may be NULL). Both
+ * twins run the same kernels, count and PointType_CMP tie order (ikd_Tree.h:57-60, applied when both out_xyz and out_d2 are given)
+ * included; the host twin only adds the copies of the queries and the results. No synchronisation, any n. */
 int liinit_map_nearest_search_device(liinit_ctx* h, const float* q_xyz, int stride_floats, int n, double max_dist, float* out_xyz,
                                      float* out_d2, int* out_cnt);
 /* liinit_cloud_download: the records are built in rec12 itself, which must be 16-byte aligned. n (host, may be NULL) and d_n (device,

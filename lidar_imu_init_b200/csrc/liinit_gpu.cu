@@ -338,6 +338,17 @@ int stage_batch(Ctx* c, const float* xyz, int stride, int n, bool dev, const flo
     return stage_points(c, xyz, stride, n);
 }
 
+// the first n device points into packed host xyz [n*3] (synchronises)
+int download_xyz(Ctx* c, const float4* src, size_t n, float* xyz) {
+    std::vector<float4> b(n);
+    CU(cudaMemcpyAsync(b.data(), src, n * sizeof(float4), cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    for (size_t i = 0; i < n; i++) {
+        xyz[3 * i] = b[i].x; xyz[3 * i + 1] = b[i].y; xyz[3 * i + 2] = b[i].z;
+    }
+    return LIINIT_OK;
+}
+
 int fetch_counters(Ctx* c) {
     CU(cudaMemcpyAsync(c->h_counters, c->d_counters, sizeof(int) * CNT_COUNT, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaMemcpyAsync(c->h_pool_top, c->M.pool_top, sizeof(unsigned long long), cudaMemcpyDeviceToHost, c->stream));
@@ -664,6 +675,17 @@ int gather_scan_state(Ctx* c) {
     return LIINIT_OK;
 }
 
+// One stable 8-bit pass of the radix sort (sort_kernels.cuh) of the pairs (k[cur], v[cur]) into (k[cur ^ 1], v[cur ^ 1]); cur then names
+// the sorted pairs. n: the element count, or the bound the launch is sized for when n_dev holds the count on the device.
+void rs_pass(Ctx* c, unsigned* const k[2], unsigned* const v[2], int& cur, int* hist, int n, const int* n_dev, int shift) {
+    const int ntiles = nblk(n, RS_TILE);
+    k_rs_hist<<<nblk(ntiles, 4), 128, 0, c->stream>>>(k[cur], n, n_dev, shift, ntiles, hist);
+    k_rs_scan<<<1, 1024, 0, c->stream>>>(256 * ntiles, hist);
+    k_rs_scatter<<<nblk(ntiles, 4), 128, 0, c->stream>>>(k[cur], v[cur], n, n_dev, shift, ntiles, hist, k[cur ^ 1], v[cur ^ 1]);
+    c->launches += 3;
+    cur ^= 1;
+}
+
 // ---- cut-frame preprocess ------------------------------------------------------------------------------------------------
 void frame_free(Ctx* c) {
     cudaFree(c->d_fr_in); cudaFree(c->d_fr_dec); cudaFree(c->d_fr_inten); cudaFree(c->d_fr_flag); cudaFree(c->d_fr_keys); cudaFree(c->d_fr_vals);
@@ -737,21 +759,16 @@ int frame_finish(Ctx* c, int n, int R, double S, int* tsum, liinit_subframe* out
     const int nb = nblk(n, LI_FR_TILE);
     k_rs_scan<<<1, 1024, 0, c->stream>>>(nb, tsum);
     k_fr_compact<<<nb, LI_FR_TILE, 0, c->stream>>>(c->d_fr_flag, n, tsum, c->d_fr_dec, nullptr, c->d_fr_keys, c->d_fr_vals, &c->d_fr_tab->V);
-    unsigned *k0 = c->d_fr_keys, *v0 = c->d_fr_vals, *k1 = c->d_rs_keys, *v1 = c->d_rs_vals;
-    const int ntiles = nblk(n, RS_TILE);
-    for (int pass = 0; pass < 4; pass++) {
-        k_rs_hist_dev<<<nblk(ntiles, 4), 128, 0, c->stream>>>(k0, &c->d_fr_tab->V, 8 * pass, ntiles, c->d_rs_hist);
-        k_rs_scan<<<1, 1024, 0, c->stream>>>(256 * ntiles, c->d_rs_hist);
-        k_rs_scatter_dev<<<nblk(ntiles, 4), 128, 0, c->stream>>>(k0, v0, &c->d_fr_tab->V, 8 * pass, ntiles, c->d_rs_hist, k1, v1);
-        unsigned* t = k0; k0 = k1; k1 = t;
-        t = v0; v0 = v1; v1 = t;
-    }
+    unsigned* const k[2] = {c->d_fr_keys, c->d_rs_keys};
+    unsigned* const v[2] = {c->d_fr_vals, c->d_rs_vals};
+    int cur = 0;
+    for (int pass = 0; pass < 4; pass++) rs_pass(c, k, v, cur, c->d_rs_hist, n, &c->d_fr_tab->V, 8 * pass);
     const int slot = (int)(c->fr_seq % LIINIT_FRAME_SLOTS);
     const size_t cap = (size_t)c->stage_pts_cap;
-    k_fr_bounds<<<1, 32, 0, c->stream>>>(v0, c->d_fr_dec, R, S, c->d_fr_tab);
-    k_fr_gather<<<nblk(n, 256), 256, 0, c->stream>>>(v0, c->d_fr_dec, c->d_fr_inten, S, c->d_fr_tab, c->d_fr_slot_pts + slot * cap,
+    k_fr_bounds<<<1, 32, 0, c->stream>>>(v[cur], c->d_fr_dec, R, S, c->d_fr_tab);
+    k_fr_gather<<<nblk(n, 256), 256, 0, c->stream>>>(v[cur], c->d_fr_dec, c->d_fr_inten, S, c->d_fr_tab, c->d_fr_slot_pts + slot * cap,
                                                      c->d_fr_slot_inten + slot * cap);
-    c->launches += 16;
+    c->launches += 4;
     CU(cudaGetLastError());
     CU(cudaMemcpyAsync(c->h_fr_tab, c->d_fr_tab, offsetof(FrameTable, sub) + (size_t)R * sizeof(FrameSub), cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
@@ -1260,6 +1277,90 @@ int liinit_map_stats(liinit_ctx* h, int* bricks, int* hash_slots, long long* poo
     return LIINIT_OK;
 }
 
+}  // extern "C"
+
+namespace {
+// liinit_map_download and its device twin: the live points as packed xyz into xyz [cap*3], their number into *d_n (both device memory)
+int map_flatten(Ctx* c, float* xyz, int cap, int* d_n) {
+    int r = fetch_counters(c);   // the brick count sizes the launch
+    if (r) return r;
+    CU(cudaMemsetAsync(d_n, 0, sizeof(int), c->stream));
+    if (c->h_counters[CNT_BRICKS] > 0)
+        k_map_flatten<<<nblk((long long)c->h_counters[CNT_BRICKS] * 32, 256), 256, 0, c->stream>>>(c->M, c->hash_slots, xyz, cap, d_n);
+    c->launches++;
+    CU(cudaGetLastError());
+    return LIINIT_OK;
+}
+
+// The 5-NN of m staged queries for both stand-alone searches: the query kernel of the context's index leaves ids in d_near_ids (the
+// search pass's hand-over buffer, free between passes) and distances in d_q_d2, both sized for one staging chunk; k_query_finish then
+// writes the outputs (device memory, any may be null).
+int query_batch(Ctx* c, const float4* pts, int m, float* out_xyz, float* out_d2, int* out_cnt) {
+    if (c->cells) {
+        const int gq = nblk(m, LI_CELLS_THREADS);
+        if (c->cells_search == 1) k_knn_cells_queries<1><<<gq, LI_CELLS_THREADS, 0, c->stream>>>(c->M, pts, m, c->d_near_ids, c->d_q_d2, c->rho2);
+        else if (c->cells_search == 2) k_knn_cells_queries<2><<<gq, LI_CELLS_THREADS, 0, c->stream>>>(c->M, pts, m, c->d_near_ids, c->d_q_d2, c->rho2);
+        else k_knn_cells_queries<3><<<gq, LI_CELLS_THREADS, 0, c->stream>>>(c->M, pts, m, c->d_near_ids, c->d_q_d2, c->rho2);
+    } else {
+        int grid = nblk((long long)m * 8, 256);
+        if (grid > c->max_blocks) grid = c->max_blocks;
+        k_knn_queries<8><<<grid, 256, 0, c->stream>>>(c->M, pts, m, c->d_near_ids, c->d_q_d2, c->rho2);
+    }
+    k_query_finish<<<nblk(m, 256), 256, 0, c->stream>>>(c->M.pool, c->d_near_ids, c->d_q_d2, m, out_xyz, out_d2, out_cnt);
+    c->launches += 2;
+    CU(cudaGetLastError());
+    return LIINIT_OK;
+}
+
+// liinit_scan_upload and its device twin (dev: body is device memory, checked by the caller)
+int scan_upload(Ctx* c, const float* body, int stride, int n, bool dev) {
+    if (n > c->cfg.max_scan_points) return fail(c, LIINIT_ERR_CAPACITY, "n exceeds max_scan_points");
+    if (stride != 3 && stride != 4 && stride != 12) return fail(c, LIINIT_ERR_INVALID, "stride_floats must be 3, 4 or 12");
+    if (stride == 4 && (!dev || aligned16(body))) {
+        CU(cudaMemcpyAsync(c->d_body, body, (size_t)n * 16, dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, c->stream));
+    } else {
+        if (!dev) {   // a host array goes through the strided staging buffer
+            const size_t nf = (size_t)n * stride;
+            if (nf > c->stage_raw_floats) return fail(c, LIINIT_ERR_CAPACITY, "scan exceeds staging capacity");
+            CU(cudaMemcpyAsync(c->d_stage_raw, body, nf * 4, cudaMemcpyHostToDevice, c->stream));
+            body = c->d_stage_raw;
+        }
+        k_repack<<<nblk(n, 256), 256, 0, c->stream>>>(body, stride, n, c->d_body);
+        c->launches++;
+    }
+    c->attached = nullptr;
+    c->attached_slot_done = false;
+    c->body_attr = false;
+    // new scan: no neighbours, nothing selected (Nearest_Points / point_selected_surf start over at iteration 0)
+    set_scan(c, n);
+    CU(cudaGetLastError());
+    return LIINIT_OK;
+}
+
+// liinit_raw_upload and its device twin (dev: pts is device memory, checked here after the layout)
+int raw_upload(Ctx* c, const float* pts, int stride, int time_index, int n, bool dev) {
+    if (stride < 3 || time_index >= stride || (time_index >= 0 && time_index < 3)) return fail(c, LIINIT_ERR_INVALID, "bad stride / time_index");
+    if (dev) {
+        int r = check_device_ptr(c, pts, "pts");
+        if (r) return r;
+    }
+    if (n > c->stage_pts_cap || (size_t)n * stride > c->stage_raw_floats) return fail(c, LIINIT_ERR_CAPACITY, "raw cloud exceeds staging capacity");
+    if (!dev) {
+        CU(cudaMemcpyAsync(c->d_stage_raw, pts, (size_t)n * stride * 4, cudaMemcpyHostToDevice, c->stream));
+        pts = c->d_stage_raw;
+    }
+    // the PointType layout (the time in curvature) brings its normals and intensity along; any other layout has none
+    c->stage_attr = stride >= 12 && time_index == 9;
+    k_repack_t<<<nblk(n, 256), 256, 0, c->stream>>>(pts, stride, time_index, n, c->d_stage_pts, c->stage_attr ? c->d_stage_attr : nullptr);
+    c->launches++;
+    c->raw_n = n;
+    CU(cudaGetLastError());
+    return LIINIT_OK;
+}
+}  // namespace
+
+extern "C" {
+
 int liinit_map_download(liinit_ctx* h, float* xyz, int cap, int* n) {
     if (!h || !n || cap < 0) return LIINIT_ERR_INVALID;
     Ctx* c = &h->c;
@@ -1268,22 +1369,16 @@ int liinit_map_download(liinit_ctx* h, float* xyz, int cap, int* n) {
     DevBuf<int> dn;
     CU(out.alloc((size_t)(cap > 0 ? cap : 1) * 3));
     CU(dn.alloc(1));
-    float* d_out = out.p;
-    int* d_n = dn.p;
-    CU(cudaMemsetAsync(d_n, 0, 4, c->stream));
-    {
-        int r = fetch_counters(c);
-        if (r) return r;
-    }
-    if (c->h_counters[CNT_BRICKS] > 0)
-        k_map_flatten<<<nblk((long long)c->h_counters[CNT_BRICKS] * 32, 256), 256, 0, c->stream>>>(c->M, c->hash_slots, d_out, cap, d_n);
-    c->launches++;
-    CU(cudaGetLastError());
+    int r = map_flatten(c, out.p, cap, dn.p);
+    if (r) return r;
     int cnt = 0;
-    CU(cudaMemcpyAsync(&cnt, d_n, 4, cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaMemcpyAsync(&cnt, dn.p, 4, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
-    int m = cnt < cap ? cnt : cap;
-    if (m > 0 && xyz) CU(cudaMemcpy(xyz, d_out, (size_t)m * 12, cudaMemcpyDeviceToHost));
+    const int m = cnt < cap ? cnt : cap;
+    if (m > 0 && xyz) {
+        CU(cudaMemcpyAsync(xyz, out.p, (size_t)m * 12, cudaMemcpyDeviceToHost, c->stream));
+        CU(cudaStreamSynchronize(c->stream));
+    }
     *n = cnt;
     return LIINIT_OK;
 }
@@ -1296,14 +1391,7 @@ int liinit_map_download_device(liinit_ctx* h, float* xyz, int cap, int* d_n) {
     if (!r) r = check_device_ptr(c, d_n, "d_n");
     if (!r && cap > 0) r = check_device_ptr(c, xyz, "xyz");
     if (r) return r;
-    r = fetch_counters(c);   // the brick count sizes the launch
-    if (r) return r;
-    CU(cudaMemsetAsync(d_n, 0, sizeof(int), c->stream));
-    if (c->h_counters[CNT_BRICKS] > 0)
-        k_map_flatten<<<nblk((long long)c->h_counters[CNT_BRICKS] * 32, 256), 256, 0, c->stream>>>(c->M, c->hash_slots, xyz, cap, d_n);
-    c->launches++;
-    CU(cudaGetLastError());
-    return LIINIT_OK;
+    return map_flatten(c, xyz, cap, d_n);
 }
 
 int liinit_map_nearest_search(liinit_ctx* h, const float* q, int stride, int n, double max_dist, float* out_xyz, float* out_d2,
@@ -1312,52 +1400,25 @@ int liinit_map_nearest_search(liinit_ctx* h, const float* q, int stride, int n, 
     Ctx* c = &h->c;
     if (max_dist != 5.0) return fail(c, LIINIT_ERR_INVALID, "only max_dist = 5 (laserMapping.cpp:980) is supported");
     CU(cudaSetDevice(c->device));
-    std::vector<int> ids((size_t)5 * (n > 0 ? n : 1));
+    // per chunk of the staging capacity: the queries are staged, searched into one device buffer (the wanted outputs of a chunk) and
+    // copied back in stream order
+    const int chunk = n < c->stage_pts_cap ? n : c->stage_pts_cap;
+    const size_t nx = out_xyz ? (size_t)chunk * 15 : 0, nd = out_d2 ? (size_t)chunk * 5 : 0, nc = out_cnt ? (size_t)chunk : 0;
+    DevBuf<float> out;
+    if (nx + nd + nc > 0) CU(out.alloc(nx + nd + nc));
+    float* d_xyz = out_xyz ? out.p : nullptr;
+    float* d_d2 = out_d2 ? out.p + nx : nullptr;
+    int* d_cnt = out_cnt ? reinterpret_cast<int*>(out.p + nx + nd) : nullptr;
     for (long long off = 0; off < n; off += c->stage_pts_cap) {
-        int m = (int)((n - off < c->stage_pts_cap) ? (n - off) : c->stage_pts_cap);
+        const int m = (int)((n - off < c->stage_pts_cap) ? (n - off) : c->stage_pts_cap);
         int r = stage_points(c, q + (size_t)off * stride, stride, m);
+        if (!r) r = query_batch(c, c->d_stage_pts, m, d_xyz, d_d2, d_cnt);
         if (r) return r;
-        DevBuf<int> bids;
-        DevBuf<float> bxyz;
-        CU(bids.alloc((size_t)m * 5));
-        CU(bxyz.alloc((size_t)m * 15));
-        int* d_ids = bids.p;
-        float* d_xyz = bxyz.p;
-        if (c->cells) {
-            const int gq = nblk(m, LI_CELLS_THREADS);
-            if (c->cells_search == 1) k_knn_cells_queries<1><<<gq, LI_CELLS_THREADS, 0, c->stream>>>(c->M, c->d_stage_pts, m, d_ids, c->d_q_d2, c->rho2);
-            else if (c->cells_search == 2) k_knn_cells_queries<2><<<gq, LI_CELLS_THREADS, 0, c->stream>>>(c->M, c->d_stage_pts, m, d_ids, c->d_q_d2, c->rho2);
-            else k_knn_cells_queries<3><<<gq, LI_CELLS_THREADS, 0, c->stream>>>(c->M, c->d_stage_pts, m, d_ids, c->d_q_d2, c->rho2);
-        } else {
-            int grid = nblk((long long)m * 8, 256);
-            if (grid > c->max_blocks) grid = c->max_blocks;
-            k_knn_queries<8><<<grid, 256, 0, c->stream>>>(c->M, c->d_stage_pts, m, d_ids, c->d_q_d2, c->rho2);
-        }
-        k_gather_xyz<<<nblk((long long)m * 5, 256), 256, 0, c->stream>>>(c->M.pool, d_ids, (long long)m * 5, d_xyz);
-        c->launches += 2;
-        CU(cudaGetLastError());
-        CU(cudaMemcpyAsync(ids.data() + (size_t)off * 5, d_ids, (size_t)m * 5 * 4, cudaMemcpyDeviceToHost, c->stream));
         if (out_xyz) CU(cudaMemcpyAsync(out_xyz + (size_t)off * 15, d_xyz, (size_t)m * 15 * 4, cudaMemcpyDeviceToHost, c->stream));
-        if (out_d2) CU(cudaMemcpyAsync(out_d2 + (size_t)off * 5, c->d_q_d2, (size_t)m * 5 * 4, cudaMemcpyDeviceToHost, c->stream));
-        CU(cudaStreamSynchronize(c->stream));
+        if (out_d2) CU(cudaMemcpyAsync(out_d2 + (size_t)off * 5, d_d2, (size_t)m * 5 * 4, cudaMemcpyDeviceToHost, c->stream));
+        if (out_cnt) CU(cudaMemcpyAsync(out_cnt + off, d_cnt, (size_t)m * 4, cudaMemcpyDeviceToHost, c->stream));
     }
-    for (int i = 0; i < n; i++) {
-        int cnt = 0;
-        for (int k = 0; k < 5; k++)
-            if (ids[(size_t)i * 5 + k] >= 0) cnt++;
-        if (out_cnt) out_cnt[i] = cnt;
-        // PointType_CMP tie order (ikd_Tree.h:57-60)
-        if (out_xyz && out_d2) {
-            for (int pass = 0; pass < 4; pass++)
-                for (int k = 0; k + 1 < cnt; k++) {
-                    size_t a = (size_t)i * 5 + k, b = a + 1;
-                    if (std::fabs(out_d2[a] - out_d2[b]) < 1e-10f && out_xyz[3 * b] < out_xyz[3 * a]) {
-                        for (int t = 0; t < 3; t++) std::swap(out_xyz[3 * a + t], out_xyz[3 * b + t]);
-                        std::swap(out_d2[a], out_d2[b]);
-                    }
-                }
-        }
-    }
+    CU(cudaStreamSynchronize(c->stream));
     return LIINIT_OK;
 }
 
@@ -1373,27 +1434,13 @@ int liinit_map_nearest_search_device(liinit_ctx* h, const float* q, int stride, 
     if (!r && out_d2) r = check_device_ptr(c, out_d2, "out_d2");
     if (!r && out_cnt) r = check_device_ptr(c, out_cnt, "out_cnt");
     if (r) return r;
-    // chunks of the staging capacity, in stream order: the ids go to d_near_ids (a hand-over inside one search pass, free between
-    // passes) and the distances to d_q_d2, both sized for one chunk; k_query_finish writes the caller's buffers
     for (long long off = 0; off < n; off += c->stage_pts_cap) {
         const int m = (int)((n - off < c->stage_pts_cap) ? (n - off) : c->stage_pts_cap);
         const float4* pts = nullptr;
         r = stage_points_device(c, q + (size_t)off * stride, stride, m, &pts);
+        if (!r) r = query_batch(c, pts, m, out_xyz ? out_xyz + (size_t)off * 15 : nullptr, out_d2 ? out_d2 + (size_t)off * 5 : nullptr,
+                                out_cnt ? out_cnt + off : nullptr);
         if (r) return r;
-        if (c->cells) {
-            const int gq = nblk(m, LI_CELLS_THREADS);
-            if (c->cells_search == 1) k_knn_cells_queries<1><<<gq, LI_CELLS_THREADS, 0, c->stream>>>(c->M, pts, m, c->d_near_ids, c->d_q_d2, c->rho2);
-            else if (c->cells_search == 2) k_knn_cells_queries<2><<<gq, LI_CELLS_THREADS, 0, c->stream>>>(c->M, pts, m, c->d_near_ids, c->d_q_d2, c->rho2);
-            else k_knn_cells_queries<3><<<gq, LI_CELLS_THREADS, 0, c->stream>>>(c->M, pts, m, c->d_near_ids, c->d_q_d2, c->rho2);
-        } else {
-            int grid = nblk((long long)m * 8, 256);
-            if (grid > c->max_blocks) grid = c->max_blocks;
-            k_knn_queries<8><<<grid, 256, 0, c->stream>>>(c->M, pts, m, c->d_near_ids, c->d_q_d2, c->rho2);
-        }
-        k_query_finish<<<nblk(m, 256), 256, 0, c->stream>>>(c->M.pool, c->d_near_ids, c->d_q_d2, m, out_xyz ? out_xyz + (size_t)off * 15 : nullptr,
-                                                            out_d2 ? out_d2 + (size_t)off * 5 : nullptr, out_cnt ? out_cnt + off : nullptr);
-        c->launches += 2;
-        CU(cudaGetLastError());
     }
     return LIINIT_OK;
 }
@@ -1402,25 +1449,7 @@ int liinit_scan_upload(liinit_ctx* h, const float* body, int stride, int n) {
     if (!h || !body || n <= 0) return LIINIT_ERR_INVALID;
     Ctx* c = &h->c;
     CU(cudaSetDevice(c->device));
-    if (n > c->cfg.max_scan_points) return fail(c, LIINIT_ERR_CAPACITY, "n exceeds max_scan_points");
-    c->attached = nullptr;
-    c->attached_slot_done = false;
-    c->body_attr = false;
-    if (stride == 4) {
-        CU(cudaMemcpyAsync(c->d_body, body, (size_t)n * 16, cudaMemcpyHostToDevice, c->stream));
-    } else if (stride == 3 || stride == 12) {
-        size_t nf = (size_t)n * stride;
-        if (nf > c->stage_raw_floats) return fail(c, LIINIT_ERR_CAPACITY, "scan exceeds staging capacity");
-        CU(cudaMemcpyAsync(c->d_stage_raw, body, nf * 4, cudaMemcpyHostToDevice, c->stream));
-        k_repack<<<nblk(n, 256), 256, 0, c->stream>>>(c->d_stage_raw, stride, n, c->d_body);
-        c->launches++;
-    } else {
-        return fail(c, LIINIT_ERR_INVALID, "stride_floats must be 3, 4 or 12");
-    }
-    // new scan: no neighbours, nothing selected (Nearest_Points / point_selected_surf start over at iteration 0)
-    set_scan(c, n);
-    CU(cudaGetLastError());
-    return LIINIT_OK;
+    return scan_upload(c, body, stride, n, false);
 }
 
 int liinit_scan_upload_device(liinit_ctx* h, const float* body, int stride, int n) {
@@ -1430,19 +1459,7 @@ int liinit_scan_upload_device(liinit_ctx* h, const float* body, int stride, int 
     int r = device_twin_check(c, stride);
     if (!r) r = check_device_ptr(c, body, "body_xyz");
     if (r) return r;
-    if (n > c->cfg.max_scan_points) return fail(c, LIINIT_ERR_CAPACITY, "n exceeds max_scan_points");
-    if (stride == 4 && aligned16(body)) {
-        CU(cudaMemcpyAsync(c->d_body, body, (size_t)n * 16, cudaMemcpyDeviceToDevice, c->stream));
-    } else {
-        k_repack<<<nblk(n, 256), 256, 0, c->stream>>>(body, stride, n, c->d_body);
-        c->launches++;
-    }
-    c->attached = nullptr;
-    c->attached_slot_done = false;
-    c->body_attr = false;
-    set_scan(c, n);
-    CU(cudaGetLastError());
-    return LIINIT_OK;
+    return scan_upload(c, body, stride, n, true);
 }
 
 int liinit_scan_attach_host(liinit_ctx* h, const float* pinned_body, int stride, int n) {
@@ -1468,16 +1485,7 @@ int liinit_raw_upload(liinit_ctx* h, const float* pts, int stride, int time_inde
     if (!h || !pts || n <= 0) return LIINIT_ERR_INVALID;
     Ctx* c = &h->c;
     CU(cudaSetDevice(c->device));
-    if (stride < 3 || time_index >= stride || (time_index >= 0 && time_index < 3)) return fail(c, LIINIT_ERR_INVALID, "bad stride / time_index");
-    if (n > c->stage_pts_cap || (size_t)n * stride > c->stage_raw_floats) return fail(c, LIINIT_ERR_CAPACITY, "raw cloud exceeds staging capacity");
-    CU(cudaMemcpyAsync(c->d_stage_raw, pts, (size_t)n * stride * 4, cudaMemcpyHostToDevice, c->stream));
-    // the PointType layout (the time in curvature) brings its normals and intensity along; any other layout has none
-    c->stage_attr = stride >= 12 && time_index == 9;
-    k_repack_t<<<nblk(n, 256), 256, 0, c->stream>>>(c->d_stage_raw, stride, time_index, n, c->d_stage_pts, c->stage_attr ? c->d_stage_attr : nullptr);
-    c->launches++;
-    c->raw_n = n;
-    CU(cudaGetLastError());
-    return LIINIT_OK;
+    return raw_upload(c, pts, stride, time_index, n, false);
 }
 
 int liinit_raw_upload_device(liinit_ctx* h, const float* pts, int stride, int time_index, int n) {
@@ -1485,16 +1493,7 @@ int liinit_raw_upload_device(liinit_ctx* h, const float* pts, int stride, int ti
     Ctx* c = &h->c;
     CU(cudaSetDevice(c->device));
     if (has_comm(c)) return fail(c, LIINIT_ERR_INVALID, "the device-pointer entry points do not take a communicator (liinit_comm_init)");
-    if (stride < 3 || time_index >= stride || (time_index >= 0 && time_index < 3)) return fail(c, LIINIT_ERR_INVALID, "bad stride / time_index");
-    int r = check_device_ptr(c, pts, "pts");
-    if (r) return r;
-    if (n > c->stage_pts_cap || (size_t)n * stride > c->stage_raw_floats) return fail(c, LIINIT_ERR_CAPACITY, "raw cloud exceeds staging capacity");
-    c->stage_attr = stride >= 12 && time_index == 9;
-    k_repack_t<<<nblk(n, 256), 256, 0, c->stream>>>(pts, stride, time_index, n, c->d_stage_pts, c->stage_attr ? c->d_stage_attr : nullptr);
-    c->launches++;
-    c->raw_n = n;
-    CU(cudaGetLastError());
-    return LIINIT_OK;
+    return raw_upload(c, pts, stride, time_index, n, true);
 }
 
 static int raw_time_range(Ctx* c) {
@@ -1615,21 +1614,20 @@ int liinit_frame_cut_pcl2(liinit_ctx* h, const void* data, const liinit_pcl2_lay
         int* ring_first = c->d_fr_ring;
         int* ring_desc = c->d_fr_ring + 256;
         int* n_surv = c->d_fr_ring + 512;
-        const int ntiles = nblk(n, RS_TILE);
         float* base = reinterpret_cast<float*>(c->d_fr_aux);
         k_rs_scan<<<1, 1024, 0, c->stream>>>(nb, tsum);
         k_fr_compact<<<nb, LI_FR_TILE, 0, c->stream>>>(c->d_fr_flag, n, tsum, c->d_fr_dec, c->d_fr_aux, c->d_fr_keys, c->d_fr_vals, n_surv);
-        k_rs_hist_dev<<<nblk(ntiles, 4), 128, 0, c->stream>>>(c->d_fr_keys, n_surv, 0, ntiles, c->d_rs_hist);
-        k_rs_scan<<<1, 1024, 0, c->stream>>>(256 * ntiles, c->d_rs_hist);
-        k_rs_scatter_dev<<<nblk(ntiles, 4), 128, 0, c->stream>>>(c->d_fr_keys, c->d_fr_vals, n_surv, 0, ntiles, c->d_rs_hist, c->d_rs_keys,
-                                                                 c->d_rs_vals);
+        unsigned* const k[2] = {c->d_fr_keys, c->d_rs_keys};
+        unsigned* const v[2] = {c->d_fr_vals, c->d_rs_vals};
+        int cur = 0;
+        rs_pass(c, k, v, cur, c->d_rs_hist, n, n_surv, 0);   // -> d_rs_keys / d_rs_vals
         k_fr_yaw_first<<<nblk(n, 256), 256, 0, c->stream>>>(c->d_rs_keys, c->d_rs_vals, n_surv, c->d_fr_dec, c->d_fr_yaw, ring_first, ring_desc);
         k_fr_yaw_base<<<nblk(n, 256), 256, 0, c->stream>>>(c->d_rs_keys, n_surv, c->d_fr_yaw, ring_first, base, ring_desc);
         k_fr_yaw_final<<<nblk(n, 256), 256, 0, c->stream>>>(c->d_rs_keys, c->d_rs_vals, n_surv, base, ring_first, ring_desc, p->N_SCANS,
                                                            p->point_filter_num, c->d_fr_dec, c->d_fr_flag, &c->d_fr_tab->err);
         k_fr_yaw_chain<<<1, 256, 0, c->stream>>>(c->d_rs_keys, c->d_rs_vals, n_surv, base, ring_first, &c->d_fr_tab->err, c->d_fr_dec);
         k_fr_tile_count<<<nb, LI_FR_TILE, 0, c->stream>>>(c->d_fr_flag, n, tsum);
-        c->launches += 10;
+        c->launches += 7;
     }
     CU(cudaGetLastError());
     return frame_finish(c, n, R, p->stamp * 1000, tsum, out, n_sub);
@@ -1683,14 +1681,7 @@ int liinit_raw_download(liinit_ctx* h, float* xyz, int cap, int* n) {
     CU(cudaSetDevice(c->device));
     *n = c->raw_n;
     int m = c->raw_n < cap ? c->raw_n : cap;
-    if (m > 0 && xyz) {
-        std::vector<float4> b(m);
-        CU(cudaStreamSynchronize(c->stream));
-        CU(cudaMemcpy(b.data(), c->d_stage_pts, (size_t)m * 16, cudaMemcpyDeviceToHost));
-        for (int i = 0; i < m; i++) {
-            xyz[3 * (size_t)i] = b[i].x; xyz[3 * (size_t)i + 1] = b[i].y; xyz[3 * (size_t)i + 2] = b[i].z;
-        }
-    }
+    if (m > 0 && xyz) return download_xyz(c, c->d_stage_pts, m, xyz);
     return LIINIT_OK;
 }
 
@@ -1723,7 +1714,6 @@ int liinit_raw_downsample(liinit_ctx* h, float leaf_size, int* n_down) {
     const int inf_pos = 0x7f800000, inf_neg = (int)0xff800000 ^ 0x7fffffff;   // ordered-int images of +inf / -inf
     const int init[8] = {inf_pos, inf_pos, inf_pos, inf_neg, inf_neg, inf_neg, 0, 0};
     CU(cudaMemcpyAsync(c->d_vg_misc, init, sizeof(init), cudaMemcpyHostToDevice, c->stream));
-    const int nb = nblk(n, 1024);
     VoxTmp V = sized_vox(c, n);
     k_vg_clear<<<nblk((long long)V.mask + 1, 256), 256, 0, c->stream>>>(V, c->d_vg_imin);
     k_vg_minmax<<<nblk(n, 256), 256, 0, c->stream>>>(c->d_stage_pts, n, c->d_vg_misc);
@@ -1731,28 +1721,17 @@ int liinit_raw_downsample(liinit_ctx* h, float leaf_size, int* n_down) {
     k_vg_link<<<nblk(n, 256), 256, 0, c->stream>>>(c->d_stage_pts, n, c->d_vg_params, V, c->d_vg_imin, c->d_vslot_of, c->d_slot_of,
                                                      c->d_vg_misc + 7);
     // one (leaf index, first point) pair per leaf, sorted by leaf index: PCL's output order
-    unsigned* k0 = reinterpret_cast<unsigned*>(c->d_flag);
-    unsigned* v0 = reinterpret_cast<unsigned*>(c->d_ins);
-    unsigned* k1 = c->d_rs_keys;
-    unsigned* v1 = c->d_rs_vals;
-    k_vg_collect<<<nblk((long long)V.mask + 1, 256), 256, 0, c->stream>>>(V, c->d_vg_imin, k0, v0, c->d_vg_misc + 6);
-    {
-        // the number of leaves is only known on the device: sort with the worst-case tile count, the kernels read the real n
-        const int ntiles = nblk(n, RS_TILE);
-        for (int pass = 0; pass < 4; pass++) {
-            k_rs_hist_dev<<<nblk(ntiles, 4), 128, 0, c->stream>>>(k0, c->d_vg_misc + 6, 8 * pass, ntiles, c->d_rs_hist);
-            k_rs_scan<<<1, 1024, 0, c->stream>>>(256 * ntiles, c->d_rs_hist);
-            k_rs_scatter_dev<<<nblk(ntiles, 4), 128, 0, c->stream>>>(k0, v0, c->d_vg_misc + 6, 8 * pass, ntiles, c->d_rs_hist, k1, v1);
-            unsigned* t = k0; k0 = k1; k1 = t;
-            t = v0; v0 = v1; v1 = t;
-        }
-    }
-    (void)nb;
-    k_vg_centroid_sorted<<<nblk(n, 256), 256, 0, c->stream>>>(c->d_stage_pts, v0, c->d_vg_misc + 6, c->d_slot_of, V, c->d_vslot_of, c->d_body,
+    unsigned* const k[2] = {reinterpret_cast<unsigned*>(c->d_flag), c->d_rs_keys};
+    unsigned* const v[2] = {reinterpret_cast<unsigned*>(c->d_ins), c->d_rs_vals};
+    k_vg_collect<<<nblk((long long)V.mask + 1, 256), 256, 0, c->stream>>>(V, c->d_vg_imin, k[0], v[0], c->d_vg_misc + 6);
+    c->launches += 5;
+    // the number of leaves is only known on the device: sort with the worst-case tile count, the kernels read the real n
+    int cur = 0;
+    for (int pass = 0; pass < 4; pass++) rs_pass(c, k, v, cur, c->d_rs_hist, n, c->d_vg_misc + 6, 8 * pass);
+    k_vg_centroid_sorted<<<nblk(n, 256), 256, 0, c->stream>>>(c->d_stage_pts, v[cur], c->d_vg_misc + 6, c->d_slot_of, V, c->d_vslot_of, c->d_body,
                                                                c->cfg.max_scan_points, c->d_vg_misc + 7, c->stage_attr ? c->d_stage_attr : nullptr,
                                                                c->d_body_attr);
-    c->launches += 12;
-    c->launches += 7;
+    c->launches++;
     CU(cudaGetLastError());
     int res[8];
     VgParams P;
@@ -1785,12 +1764,7 @@ int liinit_scan_download_body(liinit_ctx* h, float* xyz, int cap, int* n) {
     int m = c->scan_n < cap ? c->scan_n : cap;
     if (m > 0 && xyz) {
         materialize_scan(c);
-        std::vector<float4> b(m);
-        CU(cudaStreamSynchronize(c->stream));
-        CU(cudaMemcpy(b.data(), c->d_body, (size_t)m * 16, cudaMemcpyDeviceToHost));
-        for (int i = 0; i < m; i++) {
-            xyz[3 * (size_t)i] = b[i].x; xyz[3 * (size_t)i + 1] = b[i].y; xyz[3 * (size_t)i + 2] = b[i].z;
-        }
+        return download_xyz(c, c->d_body, m, xyz);
     }
     return LIINIT_OK;
 }
@@ -1831,14 +1805,11 @@ int liinit_scan_download_state(liinit_ctx* h, float* world_xyz, float* near_xyz,
         r = gather_scan_state(c);
         if (r) return r;
     }
-    CU(cudaStreamSynchronize(c->stream));
     if (world_xyz) {
-        std::vector<float4> w(n);
-        CU(cudaMemcpy(w.data(), c->d_world, (size_t)n * 16, cudaMemcpyDeviceToHost));
-        for (int i = 0; i < n; i++) {
-            world_xyz[3 * (size_t)i] = w[i].x; world_xyz[3 * (size_t)i + 1] = w[i].y; world_xyz[3 * (size_t)i + 2] = w[i].z;
-        }
+        int r = download_xyz(c, c->d_world, n, world_xyz);
+        if (r) return r;
     }
+    CU(cudaStreamSynchronize(c->stream));
     if (near_xyz || near_cnt) {   // Nearest_Points: the device keeps them as point copies (ScanDev::near_xyz, w = 1 found / 0 missing)
         std::vector<float4> nb((size_t)n * 5);
         CU(cudaMemcpy(nb.data(), c->d_near_xyz, (size_t)n * 5 * sizeof(float4), cudaMemcpyDeviceToHost));
@@ -2257,19 +2228,6 @@ int assess_check(Ctx* c) {
     return LIINIT_OK;
 }
 
-// one stable 8-bit pass of the radix sort over A.k[cur] / A.v[cur] into the other buffers
-int assess_sort_pass(Ctx* c, int& cur, int n, int shift) {
-    Ctx::Assess& A = c->A;
-    const int ntiles = nblk(n, RS_TILE);
-    k_rs_hist<<<nblk(ntiles, 4), 128, 0, c->stream>>>(A.k[cur], n, shift, ntiles, A.hist);
-    k_rs_scan<<<1, 1024, 0, c->stream>>>(256 * ntiles, A.hist);
-    k_rs_scatter<<<nblk(ntiles, 4), 128, 0, c->stream>>>(A.k[cur], A.v[cur], n, shift, ntiles, A.hist, A.k[cur ^ 1], A.v[cur ^ 1]);
-    c->launches += 3;
-    CU(cudaGetLastError());
-    cur ^= 1;
-    return LIINIT_OK;
-}
-
 // the checks liinit_assess_evaluate and liinit_assess_cloud share; a cloud takes every stored point as a query (stride 0 or 1)
 int assess_check_params(Ctx* c, const liinit_assess_params* prm, const double* R_LI, const double* T_LI, bool cloud) {
     const double r = prm->radius;
@@ -2323,18 +2281,13 @@ int assess_sort(Ctx* c, const AsGrid& G, int& cur) {
     CU(cudaGetLastError());
     // stable sort by cell key: the low word's digits, then (keys wider than 32 bits) the high word's; only the digits the box needs
     cur = 0;
-    for (int sh = 0; sh < bits && sh < 32; sh += 8) {
-        const int rc = assess_sort_pass(c, cur, n, sh);
-        if (rc) return rc;
-    }
+    for (int sh = 0; sh < bits && sh < 32; sh += 8) rs_pass(c, A.k, A.v, cur, A.hist, n, nullptr, sh);
     if (bits > 32) {
         k_rs_gather_hi<<<nblk(n, 256), 256, 0, c->stream>>>(A.key, A.v[cur], n, A.k[cur]);
         c->launches++;
-        for (int sh = 0; sh < bits - 32; sh += 8) {
-            const int rc = assess_sort_pass(c, cur, n, sh);
-            if (rc) return rc;
-        }
+        for (int sh = 0; sh < bits - 32; sh += 8) rs_pass(c, A.k, A.v, cur, A.hist, n, nullptr, sh);
     }
+    CU(cudaGetLastError());
     return LIINIT_OK;
 }
 
@@ -2663,15 +2616,7 @@ int liinit_assess_download_placed(liinit_ctx* h, float* xyz, long long cap, long
     if (!xyz) return LIINIT_OK;
     if (cap < m) return fail(c, LIINIT_ERR_CAPACITY, "cap is smaller than the number of stored points");
     CU(cudaSetDevice(c->device));
-    std::vector<float4> w((size_t)m);
-    CU(cudaMemcpyAsync(w.data(), c->A.world, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, c->stream));
-    CU(cudaStreamSynchronize(c->stream));
-    for (long long i = 0; i < m; i++) {
-        xyz[3 * i] = w[i].x;
-        xyz[3 * i + 1] = w[i].y;
-        xyz[3 * i + 2] = w[i].z;
-    }
-    return LIINIT_OK;
+    return download_xyz(c, c->A.world, (size_t)m, xyz);
 }
 
 }  // extern "C"

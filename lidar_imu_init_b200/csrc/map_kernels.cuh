@@ -722,22 +722,11 @@ __global__ void k_map_delete_boxes(MapDev M, unsigned slots, const float* __rest
     }
 }
 
-// neighbour ids (pool offsets, -1 = missing) -> packed xyz, so that downloads never ship the pool itself
-__global__ void k_gather_xyz(const float4* __restrict__ pool, const int* __restrict__ ids, long long n, float* __restrict__ out) {
-    long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    int id = ids[i];
-    float4 q = (id >= 0) ? pool[id] : make_float4(0.f, 0.f, 0.f, 0.f);
-    out[3 * i] = q.x;
-    out[3 * i + 1] = q.y;
-    out[3 * i + 2] = q.z;
-}
-
-// liinit_map_nearest_search_device, per query: the ids and distances k_knn_queries / k_knn_cells_queries left -> the caller's
-// buffers (any may be null). Count and tie order are the host twin's loop restated: the count is the number of ids >= 0, and with
-// both xyz and d2 wanted, four passes over the found ranks [0, cnt) swap neighbours whose distances differ by less than 1e-10 to
-// smaller x first (PointType_CMP, ikd_Tree.h:57-60). (tie_order of the plane kernel bubbles over all five ranks with shrinking
-// bounds; the bounds here follow the host twin, so that the two give the same points bit for bit.)
+// The stand-alone 5-NN search (both twins), per query: the ids (pool offsets, -1 = missing) and distances k_knn_queries /
+// k_knn_cells_queries left -> the outputs (any may be null), so that results never ship the pool itself. The count is the number of
+// ids >= 0. With both xyz and d2 wanted, four passes over the found ranks [0, cnt) swap neighbours whose distances differ by less than
+// 1e-10 to smaller x first: the PointType_CMP tie order (ikd_Tree.h:57-60). (Not the plane kernel's tie_order, which bubbles over all
+// five ranks with shrinking bounds.)
 __global__ void k_query_finish(const float4* __restrict__ pool, const int* __restrict__ ids, const float* __restrict__ d2, int n,
                                float* __restrict__ out_xyz, float* __restrict__ out_d2, int* __restrict__ out_cnt) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;

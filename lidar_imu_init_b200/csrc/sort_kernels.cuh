@@ -10,9 +10,13 @@
 
 #define RS_TILE 1024
 
+// The element count is n, or *n_dev when n_dev is given: the voxel grid and the frame cut learn their counts on the device and launch
+// for the bound n (ntiles = ceil(n / RS_TILE)); the tiles past the real count then do no work.
+
 // pass 1: per-tile digit histogram -> hist[digit * ntiles + tile]
-__global__ void k_rs_hist(const unsigned* __restrict__ keys, int n, int shift, int ntiles, int* __restrict__ hist) {
+__global__ void k_rs_hist(const unsigned* __restrict__ keys, int n, const int* __restrict__ n_dev, int shift, int ntiles, int* __restrict__ hist) {
     __shared__ int s_cnt[4][256];
+    if (n_dev) n = *n_dev;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int tile = blockIdx.x * 4 + warp;
     for (int d = lane; d < 256; d += 32) s_cnt[warp][d] = 0;
@@ -62,9 +66,10 @@ __global__ void k_rs_scan(int m, int* __restrict__ a) {
 }
 
 // pass 3: stable scatter
-__global__ void k_rs_scatter(const unsigned* __restrict__ keys, const unsigned* __restrict__ vals, int n, int shift, int ntiles,
-                             const int* __restrict__ hist, unsigned* __restrict__ keys_out, unsigned* __restrict__ vals_out) {
+__global__ void k_rs_scatter(const unsigned* __restrict__ keys, const unsigned* __restrict__ vals, int n, const int* __restrict__ n_dev, int shift,
+                             int ntiles, const int* __restrict__ hist, unsigned* __restrict__ keys_out, unsigned* __restrict__ vals_out) {
     __shared__ int s_off[4][256];
+    if (n_dev) n = *n_dev;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int tile = blockIdx.x * 4 + warp;
     if (tile < ntiles)
@@ -98,50 +103,4 @@ __global__ void k_rs_gather_hi(const unsigned long long* __restrict__ keys64, co
                                unsigned* __restrict__ keys_out) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) keys_out[i] = (unsigned)(keys64[vals[i]] >> 32);
-}
-
-// variants whose element count lives in device memory (the voxel grid learns the number of leaves on the device)
-__global__ void k_rs_hist_dev(const unsigned* __restrict__ keys, const int* __restrict__ n_dev, int shift, int ntiles, int* __restrict__ hist) {
-    __shared__ int s_cnt[4][256];
-    const int n = *n_dev;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int tile = blockIdx.x * 4 + warp;
-    for (int d = lane; d < 256; d += 32) s_cnt[warp][d] = 0;
-    __syncwarp();
-    if (tile < ntiles) {
-        const int lo = tile * RS_TILE, hi = min(n, lo + RS_TILE);
-        for (int i = lo + lane; i < hi; i += 32) atomicAdd(&s_cnt[warp][(keys[i] >> shift) & 255u], 1);
-        __syncwarp();
-        for (int d = lane; d < 256; d += 32) hist[d * ntiles + tile] = s_cnt[warp][d];
-    }
-}
-
-__global__ void k_rs_scatter_dev(const unsigned* __restrict__ keys, const unsigned* __restrict__ vals, const int* __restrict__ n_dev, int shift,
-                                 int ntiles, const int* __restrict__ hist, unsigned* __restrict__ keys_out, unsigned* __restrict__ vals_out) {
-    __shared__ int s_off[4][256];
-    const int n = *n_dev;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int tile = blockIdx.x * 4 + warp;
-    if (tile < ntiles)
-        for (int d = lane; d < 256; d += 32) s_off[warp][d] = hist[d * ntiles + tile];
-    __syncwarp();
-    if (tile >= ntiles) return;
-    const int lo = tile * RS_TILE, hi = min(n, lo + RS_TILE);
-    for (int base = lo; base < hi; base += 32) {
-        const int i = base + lane;
-        const bool valid = i < hi;
-        unsigned k = valid ? keys[i] : 0u, v = valid ? vals[i] : 0u;
-        unsigned d = valid ? ((k >> shift) & 255u) : 256u + lane;
-        unsigned peers = __match_any_sync(LI_FULL, d);
-        int rank = __popc(peers & ((1u << lane) - 1u));
-        int off = 0;
-        if (valid) off = s_off[warp][d] + rank;
-        __syncwarp();
-        if (valid && rank == 0) s_off[warp][d] += __popc(peers);
-        __syncwarp();
-        if (valid) {
-            keys_out[off] = k;
-            vals_out[off] = v;
-        }
-    }
 }
