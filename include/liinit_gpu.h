@@ -383,6 +383,47 @@ int liinit_assess_download_placed(liinit_ctx* h, float* xyz, long long cap, long
 int liinit_assess_cloud(liinit_ctx* h, const liinit_assess_params* p, const double R_LI[9], const double T_LI[3], double leaf, float* rec8,
                         long long cap_records, long long* n, liinit_assess_result* totals);
 
+/* The timed store (DESIGN.md section 4d): it also keeps what the IMU undistortion of a scan needs, so an evaluation can redo it for a
+ * candidate extrinsic and a candidate time lag. A timed scan is one whose staged cloud was held (liinit_assess_hold) before
+ * liinit_raw_undistort_imu and appended with liinit_assess_append_timed: its raw points (xyz, time [ms]), its pose table and the
+ * propagated state of that call. Every other stored scan is untimed and is placed from its stored points at every lag. The stored
+ * points, their order and everything liinit_assess_evaluate / _cloud / _download return are those of the plain store. */
+#define LIINIT_ASSESS_MAX_POSE_ROWS (1ll << 30)
+typedef struct {
+    const double* poses;  /* npose x 22 doubles (Pose6D), host memory, as passed to liinit_raw_undistort_imu */
+    int npose;            /* 2 <= npose <= LIINIT_MAX_IMU_POSES */
+    int reserved;
+    double rot[9], pos[3];    /* the propagated state passed to liinit_raw_undistort_imu: rot_end, pos_end ... */
+    double R_LI[9], T_LI[3];  /* ... and its extrinsic */
+    double vel[3];            /* the propagated vel_end */
+} liinit_assess_timing;
+/* liinit_assess_reserve, plus a raw-point buffer (16 bytes per point), a timing record per scan (about 400 bytes) and a pool of
+ * max_pose_rows pose rows (176 bytes each). Calling it (or liinit_assess_reserve) again clears the store. LIINIT_ERR_INVALID also for
+ * max_pose_rows outside [2, LIINIT_ASSESS_MAX_POSE_ROWS]. */
+int liinit_assess_reserve_timed(liinit_ctx* h, long long max_points, int max_scans, long long max_pose_rows);
+/* Holds the staged raw cloud for the next liinit_assess_append_timed: a device-to-device copy behind the stored points, no
+ * synchronisation. Call it between staging the cloud and liinit_raw_undistort_imu. Any later staging call (raw upload, frame stage,
+ * a map or scan upload) or append ends the hold. LIINIT_ERR_INVALID when no raw cloud is staged or the store is not timed. */
+int liinit_assess_hold(liinit_ctx* h);
+/* liinit_assess_append (the staged, undistorted cloud with the posterior pose and extrinsic), and commits the held raw points, the
+ * pose table and the prior state *t. No room for the points or the scan: skipped as by liinit_assess_append. No room in the pose pool:
+ * stored as an untimed scan. LIINIT_ERR_INVALID when the store is not timed, no hold of the current staged cloud exists, the held and
+ * staged clouds differ in size, or t->npose is outside [2, LIINIT_MAX_IMU_POSES]. In a timed store, liinit_assess_append stores an
+ * untimed scan. */
+int liinit_assess_append_timed(liinit_ctx* h, const double rot_end[9], const double pos_end[3], const double R_LI[9], const double T_LI[3],
+                               const liinit_assess_timing* t, int* appended);
+/* Timed and untimed stored scans and pose rows in use (any pointer may be NULL). LIINIT_ERR_INVALID for a store that is not timed. */
+int liinit_assess_timing_info(liinit_ctx* h, int* timed_scans, int* untimed_scans, long long* pose_rows);
+/* liinit_assess_evaluate with every timed scan re-undistorted for the candidate extrinsic (as_run: the prior extrinsic for the
+ * undistortion, each scan's posterior one for the placement) and the lag shift [s]: the candidate's total lag is the run's + lag_shift,
+ * so a point at tau [ms] is undistorted at t = tau / 1000 + lag_shift in the run's table, head row as liinit_raw_undistort_imu's
+ * (none: untouched at lag_shift 0, row 0 otherwise), towards rot_end Exp(gyr_last, lag_shift) and pos_end + vel_end lag_shift +
+ * 1/2 acc_last lag_shift^2 (the table's last row). At lag_shift 0 as-run it is bit-equal to liinit_assess_evaluate as-run.
+ * liinit_assess_download / _download_placed then return this evaluation's values. Errors as liinit_assess_evaluate, and
+ * LIINIT_ERR_INVALID for a store that is not timed or a non-finite lag_shift. */
+int liinit_assess_evaluate_timed(liinit_ctx* h, const liinit_assess_params* p, const double R_LI[9], const double T_LI[3], double lag_shift,
+                                 liinit_assess_result* out);
+
 #ifdef __cplusplus
 }
 #endif

@@ -9,6 +9,11 @@ that axis down as far as this measure can tell. This is a report, not a verdict 
 
 write_cloud shows where the as-run map is blurred: every stored point scored (LiInitGpu.assess_cloud), thinned to leaves on the device,
 as a PCD that a viewer colours by entropy.
+
+A timed assessment (Assessment(timed=True)) also keeps each LIO scan's raw cloud, IMU pose table and propagated state, so that every
+evaluation re-undistorts the scans for its candidate (LiInitGpu.assess_evaluate_timed). sweep_time scores the 14 candidates that way
+and a lag profile: the final extrinsic at lag shifts of k * LAG_STEP_MS, |k| <= LAG_STEPS. The lag is `constrained` when both one-step
+shifts score a higher MME than the run's lag, `flat` otherwise.
 """
 from __future__ import annotations
 
@@ -23,6 +28,9 @@ MIN_NEIGHBORS = 10
 MAX_POINTS = 30_000_000
 MAX_SCANS = 1 << 16
 CLOUD_LEAF = 0.1        # leaf edge of the assessment cloud [m]; 0: one record per stored point
+MAX_POSE_ROWS = 1 << 20  # IMU pose rows a timed store keeps (about 87 min of a 200 Hz IMU)
+LAG_STEP_MS = 2.0       # lag profile step [ms]
+LAG_STEPS = 10          # lag profile: shifts -LAG_STEPS .. LAG_STEPS steps
 AXES = ("x", "y", "z")
 NOTHING = "nothing to assess: no LIO scan was stored (LI-Init did not trigger, or the run ended at the hand-over)\n"
 
@@ -65,15 +73,29 @@ def verdicts(rows) -> dict:
 class Assessment:
     """The store of one run's LIO scans on a context and the sweep over it."""
 
-    def __init__(self, gpu, max_points=MAX_POINTS, radius=RADIUS, min_neighbors=MIN_NEIGHBORS, max_scans=MAX_SCANS):
+    def __init__(self, gpu, max_points=MAX_POINTS, radius=RADIUS, min_neighbors=MIN_NEIGHBORS, max_scans=MAX_SCANS, timed=False,
+                 max_pose_rows=MAX_POSE_ROWS):
         if not (radius > 0 and math.isfinite(radius)):
             raise ValueError(f"assessment radius {radius!r}: must be positive")
         self.g, self.radius, self.min_neighbors = gpu, float(radius), int(min_neighbors)
-        self.g.assess_reserve(int(max_points), int(max_scans))
+        self.timed = bool(timed)
+        if self.timed:
+            self.g.assess_reserve_timed(int(max_points), int(max_scans), int(max_pose_rows))
+        else:
+            self.g.assess_reserve(int(max_points), int(max_scans))
         self.final = None   # (R_LI, T_LI) of the last stored scan
 
     def append(self, rot_end, pos_end, R_LI, T_LI):
         if self.g.assess_append(rot_end, pos_end, R_LI, T_LI):
+            self.final = (np.array(R_LI, float).reshape(3, 3), np.array(T_LI, float).reshape(3))
+
+    def append_timed(self, rot_end, pos_end, R_LI, T_LI, poses, prior_state):
+        """append for a scan undistorted from the IMU pose table `poses` with the propagated state prior_state (liinit_state layout;
+        its raw cloud was held by LiInitGpu.assess_hold)."""
+        from . import host
+        R, p, rli, tli = host.state_pose(prior_state)
+        prior = (R, p, rli, tli, np.asarray(prior_state, float)[24:27])
+        if self.g.assess_append_timed(rot_end, pos_end, R_LI, T_LI, poses, prior):
             self.final = (np.array(R_LI, float).reshape(3, 3), np.array(T_LI, float).reshape(3))
 
     def sweep(self, dtheta_deg=DTHETA_DEG, dt=DT_M) -> list:
@@ -84,10 +106,32 @@ class Assessment:
             out.append((name, self.final[0] if R is None else R, self.final[1] if T is None else T, res))
         return out
 
+    def sweep_time(self, dtheta_deg=DTHETA_DEG, dt=DT_M, step_ms=LAG_STEP_MS, steps=LAG_STEPS):
+        """Timed store: ([(name, R_LI, T_LI, result)] of the 14 candidates re-undistorted at the run's lag, [(shift_ms, result)] of the
+        final extrinsic at lag shifts k * step_ms, k = -steps .. steps)."""
+        ev = lambda R, T, d: self.g.assess_evaluate_timed(R, T, d, radius=self.radius, min_neighbors=self.min_neighbors,  # noqa: E731
+                                                          as_run=R is None)
+        rows = []
+        for name, R, T in candidates(*self.final, dtheta_deg=dtheta_deg, dt=dt):
+            rows.append((name, self.final[0] if R is None else R, self.final[1] if T is None else T, ev(R, T, 0.0)))
+        prof = [(k * step_ms, ev(self.final[0], self.final[1], k * step_ms / 1000.0)) for k in range(-steps, steps + 1)]
+        return rows, prof
+
     def report(self) -> str:
         if self.final is None:
             return NOTHING
         return report_text(self.g.assess_info(), self.radius, self.min_neighbors, self.sweep())
+
+    def report_time(self, lag: float) -> str:
+        """result/assessment_time.txt of a timed store; lag: the run's total IMU-to-LiDAR time lag [s]."""
+        if self.final is None:
+            return NOTHING
+        rows, prof = self.sweep_time()
+        return time_report_text(self.g.assess_info(), self.g.assess_timing_info(), self.radius, self.min_neighbors, rows, prof, lag)
+
+    def write_time(self, path: str, lag: float):
+        with open(path, "w") as f:
+            f.write(self.report_time(lag))
 
     def write(self, path: str):
         with open(path, "w") as f:
@@ -140,3 +184,48 @@ def parse_report(text: str) -> dict:
         f = line.split()
         axes[f[0]] = (f[1], float(f[2]), float(f[3]))
     return {"header": header, "rows": rows, "axes": axes}
+
+
+def lag_verdict(profile) -> tuple:
+    """(verdict, best shift [ms]) of a lag profile [(shift_ms, result)] with shift 0 in the middle: `constrained` when both one-step
+    shifts score a higher MME than shift 0; the best shift has the lowest MME (the first of equals)."""
+    m = {s: r["mme"] for s, r in profile}
+    k = [s for s, _ in profile]
+    i0 = k.index(0.0)
+    v = "constrained" if m[k[i0 - 1]] > m[0.0] and m[k[i0 + 1]] > m[0.0] else "flat"
+    best = min((s for s in k if m[s] == m[s]), key=lambda s: m[s], default=0.0)   # (NaN: no valid query)
+    return v, best
+
+
+def time_report_text(info: dict, timing: dict, radius: float, min_neighbors: int, rows: list, profile: list, lag: float,
+                     dtheta_deg=DTHETA_DEG, dt=DT_M) -> str:
+    """result/assessment_time.txt: a header line (timed / untimed scans, pose rows, the run's lag), the 14 re-undistorted candidates in
+    assessment.txt's format, a column line and one row per lag shift, and the lag line."""
+    lines = [f"timed_scans {timing['timed_scans']} untimed_scans {timing['untimed_scans']} pose_rows {timing['pose_rows']} "
+             f"lag_ms {lag * 1000.0:.6f} lag_step_ms {profile[1][0] - profile[0][0]:.6f}",
+             report_text(info, radius, min_neighbors, rows, dtheta_deg, dt).rstrip("\n"),
+             "%10s %11s %10s %10s %10s %15s %15s" % ("shift_ms", "lag_ms", "valid", "sparse", "degenerate", "mme", "mpv")]
+    for s, r in profile:
+        lines.append("%10.3f %11.6f %10d %10d %10d %15.9f %15.9e" % (s, lag * 1000.0 + s, r["valid"], r["sparse"], r["degenerate"], r["mme"],
+                                                                   r["mpv"]))
+    v, best = lag_verdict(profile)
+    lines.append(f"lag {v} best_shift_ms {best:.3f}")
+    return "\n".join(lines) + "\n"
+
+
+def parse_time_report(text: str) -> dict:
+    """The inverse of time_report_text: {"header": {...}, "assessment": parse_report's dict of the 14 candidates, "profile":
+    [{shift_ms, lag_ms, valid, sparse, degenerate, mme, mpv}], "lag": (verdict, best shift [ms])}, or {"nothing": True}."""
+    if text == NOTHING:
+        return {"nothing": True}
+    ls = text.splitlines()
+    h = ls[0].split()
+    header = {h[i]: float(h[i + 1]) if "." in h[i + 1] else int(h[i + 1]) for i in range(0, len(h), 2)}
+    rep = parse_report("\n".join(ls[1:23]) + "\n")
+    cols = ls[23].split()
+    prof = []
+    for line in ls[24:-1]:
+        prof.append({c: (int(x) if c in ("valid", "sparse", "degenerate") else float(x)) for c, x in zip(cols, line.split())})
+    f = ls[-1].split()
+    assert f[0] == "lag" and f[2] == "best_shift_ms", ls[-1]
+    return {"header": header, "assessment": rep, "profile": prof, "lag": (f[1], float(f[3]))}

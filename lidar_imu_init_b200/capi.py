@@ -51,6 +51,11 @@ class AssessResult(C.Structure):   # liinit_assess_result
                 ("sparse", C.c_longlong), ("degenerate", C.c_longlong), ("mme", C.c_double), ("mpv", C.c_double)]
 
 
+class AssessTiming(C.Structure):   # liinit_assess_timing
+    _fields_ = [("poses", C.c_void_p), ("npose", C.c_int), ("reserved", C.c_int), ("rot", C.c_double * 9), ("pos", C.c_double * 3),
+                ("R_LI", C.c_double * 9), ("T_LI", C.c_double * 3), ("vel", C.c_double * 3)]
+
+
 ASSESS_MAX_QUERIES = 2_000_000   # LIINIT_ASSESS_MAX_QUERIES
 
 
@@ -88,7 +93,8 @@ SYMBOLS = [
     "liinit_get_stream", "liinit_map_build_device", "liinit_map_add_points_device", "liinit_scan_upload_device", "liinit_raw_upload_device",
     "liinit_map_nearest_search_device", "liinit_cloud_download_device", "liinit_map_download_device",
     "liinit_assess_reserve", "liinit_assess_append", "liinit_assess_info", "liinit_assess_evaluate", "liinit_assess_download",
-    "liinit_assess_download_placed", "liinit_assess_cloud",
+    "liinit_assess_download_placed", "liinit_assess_cloud", "liinit_assess_reserve_timed", "liinit_assess_hold", "liinit_assess_append_timed",
+    "liinit_assess_timing_info", "liinit_assess_evaluate_timed",
 ]
 
 
@@ -180,7 +186,13 @@ def set_assess_argtypes(L):
     L.liinit_assess_download_placed.argtypes = [vp, vp, C.c_longlong, C.POINTER(C.c_longlong)]
     L.liinit_assess_cloud.argtypes = [vp, C.POINTER(AssessParams), vp, vp, C.c_double, vp, C.c_longlong, C.POINTER(C.c_longlong),
                                       C.POINTER(AssessResult)]
-    for s in ("reserve", "append", "info", "evaluate", "download", "download_placed", "cloud"):
+    L.liinit_assess_reserve_timed.argtypes = [vp, C.c_longlong, C.c_int, C.c_longlong]
+    L.liinit_assess_hold.argtypes = [vp]
+    L.liinit_assess_append_timed.argtypes = [vp, _f64, _f64, _f64, _f64, C.POINTER(AssessTiming), C.POINTER(C.c_int)]
+    L.liinit_assess_timing_info.argtypes = [vp, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_longlong)]
+    L.liinit_assess_evaluate_timed.argtypes = [vp, C.POINTER(AssessParams), vp, vp, C.c_double, C.POINTER(AssessResult)]
+    for s in ("reserve", "append", "info", "evaluate", "download", "download_placed", "cloud", "reserve_timed", "hold", "append_timed",
+              "timing_info", "evaluate_timed"):
         getattr(L, "liinit_assess_" + s).restype = C.c_int
 
 
@@ -687,6 +699,44 @@ class LiInitGpu:
         out = AssessResult()
         self._ck(self.L.liinit_assess_cloud(self.h, C.byref(P), _ptr(R), _ptr(T), float(leaf), _ptr(rec), n.value, C.byref(n), C.byref(out)))
         return rec[:n.value], {k: getattr(out, k) for k, _ in AssessResult._fields_}
+
+    def assess_reserve_timed(self, max_points: int, max_scans: int, max_pose_rows: int):
+        """Allocate (or clear) a timed store: the plain store plus the raw points and IMU pose tables of the timed scans."""
+        self._ck(self.L.liinit_assess_reserve_timed(self.h, int(max_points), int(max_scans), int(max_pose_rows)))
+
+    def assess_hold(self):
+        """Hold the staged raw cloud for the next assess_append_timed (call it before the IMU undistortion)."""
+        self._ck(self.L.liinit_assess_hold(self.h))
+
+    def assess_append_timed(self, rot_end, pos_end, R_LI, T_LI, poses, prior) -> bool:
+        """assess_append, plus the held raw cloud, its pose table (npose x 22, as given to raw_undistort_imu) and the propagated state
+        of that call, prior = (rot_end, pos_end, R_LI, T_LI, vel_end). False when the store had no room (the scan is skipped)."""
+        P = np.ascontiguousarray(poses, np.float64).reshape(-1, 22)
+        t = AssessTiming()
+        t.poses = P.ctypes.data
+        t.npose = len(P)
+        for name, v, k in zip(("rot", "pos", "R_LI", "T_LI", "vel"), prior, (9, 3, 9, 3, 3)):
+            getattr(t, name)[:] = [float(x) for x in np.asarray(v, np.float64).reshape(k)]
+        ok = C.c_int(0)
+        self._ck(self.L.liinit_assess_append_timed(self.h, np.ascontiguousarray(rot_end, np.float64).reshape(9),
+                                                   np.ascontiguousarray(pos_end, np.float64).reshape(3), np.ascontiguousarray(R_LI, np.float64).reshape(9),
+                                                   np.ascontiguousarray(T_LI, np.float64).reshape(3), C.byref(t), C.byref(ok)))
+        return bool(ok.value)
+
+    def assess_timing_info(self) -> dict:
+        a, b, r = C.c_int(0), C.c_int(0), C.c_longlong(0)
+        self._ck(self.L.liinit_assess_timing_info(self.h, C.byref(a), C.byref(b), C.byref(r)))
+        return dict(timed_scans=a.value, untimed_scans=b.value, pose_rows=r.value)
+
+    def assess_evaluate_timed(self, R_LI=None, T_LI=None, lag_shift: float = 0.0, radius: float = 0.3, min_neighbors: int = 10,
+                              query_stride: int = 0, as_run: bool = False) -> dict:
+        """assess_evaluate with the timed scans re-undistorted for the candidate extrinsic and the lag shift [s]."""
+        P = AssessParams(float(radius), int(min_neighbors), int(query_stride), int(bool(as_run)), 0)
+        R = None if R_LI is None else np.ascontiguousarray(R_LI, np.float64).reshape(9)
+        T = None if T_LI is None else np.ascontiguousarray(T_LI, np.float64).reshape(3)
+        out = AssessResult()
+        self._ck(self.L.liinit_assess_evaluate_timed(self.h, C.byref(P), _ptr(R), _ptr(T), float(lag_shift), C.byref(out)))
+        return {k: getattr(out, k) for k, _ in AssessResult._fields_}
 
     def knn_index(self) -> int:
         """1 = LIINIT_KNN_BRICKS (lockstep groups over whole bricks), 2 = LIINIT_KNN_CELLS (cell directory, thread per point)."""

@@ -52,38 +52,36 @@ __global__ void k_as_store(const float4* __restrict__ stage, int n, int scan, Po
     dst[i] = make_float4(p.x, p.y, p.z, __int_as_float(scan));
 }
 
-// place: every stored point with its scan's pose and the candidate extrinsic (as_run: the scan's own); box[0..2] min cell, [3..5] max
-// cell (atomics, initialised to INT_MAX / INT_MIN by the caller), box[6] = 1 when a point lies outside the cell range
-__global__ void k_as_place(const float4* __restrict__ pts, const PoseD* __restrict__ poses, int n, int as_run, PoseD cand, double edge,
-                           float4* __restrict__ world, int* __restrict__ box) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    int c[3] = {0x7fffffff, 0x7fffffff, 0x7fffffff}, C[3] = {-0x7fffffff - 1, -0x7fffffff - 1, -0x7fffffff - 1};
-    int bad = 0;
-    if (i < n) {
-        const float4 p = pts[i];
-        const PoseD& S = poses[__float_as_int(p.w)];
-        PoseD P = cand;
+// the placement pose of a stored point of scan S: the scan's rot_end / pos_end with the candidate extrinsic (as_run: the scan's own)
+__device__ __forceinline__ PoseD li_as_pose(const PoseD& S, int as_run, const PoseD& cand) {
+    PoseD P = cand;
 #pragma unroll
-        for (int k = 0; k < 9; k++) P.R[k] = S.R[k];
+    for (int k = 0; k < 9; k++) P.R[k] = S.R[k];
 #pragma unroll
-        for (int k = 0; k < 3; k++) P.p[k] = S.p[k];
-        if (as_run) {
+    for (int k = 0; k < 3; k++) P.p[k] = S.p[k];
+    if (as_run) {
 #pragma unroll
-            for (int k = 0; k < 9; k++) P.RLI[k] = S.RLI[k];
+        for (int k = 0; k < 9; k++) P.RLI[k] = S.RLI[k];
 #pragma unroll
-            for (int k = 0; k < 3; k++) P.TLI[k] = S.TLI[k];
-        }
-        float w[3];
-        li_body_to_world(P, p.x, p.y, p.z, w[0], w[1], w[2]);
-        world[i] = make_float4(w[0], w[1], w[2], 0.f);
-#pragma unroll
-        for (int a = 0; a < 3; a++) {
-            bool ok;
-            const int v = li_as_cell(w[a], edge, ok);
-            bad |= ok ? 0 : 1;
-            if (ok) c[a] = C[a] = v;
-        }
+        for (int k = 0; k < 3; k++) P.TLI[k] = S.TLI[k];
     }
+    return P;
+}
+
+// the cells of a placed point: c / C take it as the thread's min / max cell; bad = 1 when it lies outside the cell range
+__device__ __forceinline__ void li_as_cells(const float w[3], double edge, int c[3], int C[3], int& bad) {
+#pragma unroll
+    for (int a = 0; a < 3; a++) {
+        bool ok;
+        const int v = li_as_cell(w[a], edge, ok);
+        bad |= ok ? 0 : 1;
+        if (ok) c[a] = C[a] = v;
+    }
+}
+
+// the warp's min / max cells and bad flag into box[0..2] min cell, [3..5] max cell (atomics, initialised to INT_MAX / INT_MIN by the
+// caller), box[6] = 1 when a point lies outside the cell range; every lane of the warp calls it
+__device__ __forceinline__ void li_as_box(int c[3], int C[3], int bad, int* __restrict__ box) {
     for (int o = 16; o >= 1; o >>= 1) {
 #pragma unroll
         for (int a = 0; a < 3; a++) {
@@ -100,6 +98,23 @@ __global__ void k_as_place(const float4* __restrict__ pts, const PoseD* __restri
         }
         if (bad) box[6] = 1;
     }
+}
+
+// place: every stored point with its scan's pose and the candidate extrinsic (as_run: the scan's own); the cell box as li_as_box
+__global__ void k_as_place(const float4* __restrict__ pts, const PoseD* __restrict__ poses, int n, int as_run, PoseD cand, double edge,
+                           float4* __restrict__ world, int* __restrict__ box) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    int c[3] = {0x7fffffff, 0x7fffffff, 0x7fffffff}, C[3] = {-0x7fffffff - 1, -0x7fffffff - 1, -0x7fffffff - 1};
+    int bad = 0;
+    if (i < n) {
+        const float4 p = pts[i];
+        const PoseD P = li_as_pose(poses[__float_as_int(p.w)], as_run, cand);
+        float w[3];
+        li_body_to_world(P, p.x, p.y, p.z, w[0], w[1], w[2]);
+        world[i] = make_float4(w[0], w[1], w[2], 0.f);
+        li_as_cells(w, edge, c, C, bad);
+    }
+    li_as_box(c, C, bad, box);
 }
 
 // keys of the placed points (the cells are computed exactly as in k_as_place) and the identity permutation for the sort

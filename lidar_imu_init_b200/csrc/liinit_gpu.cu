@@ -31,6 +31,7 @@
 #include "preprocess_kernels.cuh"
 #include "output_kernels.cuh"
 #include "assess_kernels.cuh"
+#include "assess_time_kernels.cuh"
 
 #ifndef LI_CELLS_MINB
 #define LI_CELLS_MINB 6
@@ -123,6 +124,7 @@ struct Ctx {
     int* d_vg_misc = nullptr;      // [0..5] min/max (ordered ints), [6] out count, [7] error bits
     VgParams* d_vg_params = nullptr;
     int raw_n = 0;                          // raw (not yet downsampled) cloud staged in d_stage_pts, w = time [ms]
+    long long stage_seq = 0;                // bumped by every staging call (a hold, liinit_assess_hold, is of one staged cloud)
     unsigned long long* d_tmin_idx = nullptr;
     double* d_poses = nullptr;              // IMU pose table for the undistortion (<= LIINIT_MAX_IMU_POSES x 22 doubles)
     VoxTmp V{};
@@ -233,6 +235,18 @@ struct Ctx {
         int* box = nullptr;
         AsTotals* tot = nullptr;
         unsigned* ticket = nullptr;
+        // timed store (liinit_assess_reserve_timed, assess_time_kernels.cuh): raw points by stored index (only a timed scan's are
+        // used), per scan its pose table and prior state, the pose pool, and per scan the undistortion target of an evaluation
+        bool timed = false;
+        float4* raw = nullptr;
+        AtScan* at = nullptr;
+        PoseD* at_end = nullptr;
+        double* pool = nullptr;
+        long long pool_cap = 0, pool_rows = 0;   // pose rows
+        int timed_scans = 0, untimed_scans = 0;
+        long long hold_seq = -1;   // stage_seq of the held cloud (-1: no hold) ...
+        int hold_n = 0;            // ... its points ...
+        long long hold_at = 0;     // ... and the stored-point count it was copied behind
     } A;
 };
 
@@ -267,6 +281,7 @@ int fail(Ctx* c, int code, const std::string& msg) {
 int stage_points(Ctx* c, const float* xyz, int stride, int n) {
     if (n > c->stage_pts_cap) return fail(c, LIINIT_ERR_CAPACITY, "batch exceeds staging capacity");
     c->raw_n = 0;   // the staging buffer is shared with the raw-scan front end
+    c->stage_seq++;
     if (stride == 4) {
         CU(cudaMemcpyAsync(c->d_stage_pts, xyz, (size_t)n * 16, cudaMemcpyHostToDevice, c->stream));
         return LIINIT_OK;
@@ -320,6 +335,7 @@ bool aligned16(const void* p) { return ((size_t)p & 15) == 0; }
 int stage_points_device(Ctx* c, const float* xyz, int stride, int n, const float4** pts) {
     if (n > c->stage_pts_cap) return fail(c, LIINIT_ERR_CAPACITY, "batch exceeds staging capacity");
     c->raw_n = 0;   // as stage_points: the staging buffer is shared with the raw-scan front end
+    c->stage_seq++;
     if (stride == 4 && aligned16(xyz)) {
         *pts = reinterpret_cast<const float4*>(xyz);
         return LIINIT_OK;
@@ -806,6 +822,7 @@ void assess_free(Ctx* c) {
     cudaFree(A.k[0]); cudaFree(A.v[0]); cudaFree(A.v[1]); cudaFree(A.hist); cudaFree(A.tc); cudaFree(A.tq); cudaFree(A.tt);
     cudaFree(A.cell_start); cudaFree(A.cell_key); cudaFree(A.cell_q0); cudaFree(A.qlist); cudaFree(A.tasks); cudaFree(A.qn); cudaFree(A.qh);
     cudaFree(A.qv); cudaFree(A.box); cudaFree(A.tot); cudaFree(A.ticket);
+    cudaFree(A.raw); cudaFree(A.at); cudaFree(A.at_end); cudaFree(A.pool);
     A = Ctx::Assess{};
 }
 
@@ -1354,6 +1371,7 @@ int raw_upload(Ctx* c, const float* pts, int stride, int time_index, int n, bool
     k_repack_t<<<nblk(n, 256), 256, 0, c->stream>>>(pts, stride, time_index, n, c->d_stage_pts, c->stage_attr ? c->d_stage_attr : nullptr);
     c->launches++;
     c->raw_n = n;
+    c->stage_seq++;
     CU(cudaGetLastError());
     return LIINIT_OK;
 }
@@ -1647,6 +1665,7 @@ int liinit_frame_stage(liinit_ctx* h, long long handle) {
     CU(cudaGetLastError());
     c->stage_attr = true;
     c->raw_n = s->n;
+    c->stage_seq++;
     return LIINIT_OK;
 }
 
@@ -2243,15 +2262,21 @@ int assess_check_params(Ctx* c, const liinit_assess_params* prm, const double* R
     return LIINIT_OK;
 }
 
-// k_as_place into A.world, then the grid of cubic cells of edge `edge` over the placed bounding box (one synchronisation); leaf: the
-// cells are the leaves of a cloud
-int assess_place(Ctx* c, int as_run, const PoseD& cand, double edge, bool leaf, AsGrid& G) {
+// k_as_place into A.world (lag: the timed placement, k_at_scan_end + k_at_place, at lag shift *lag), then the grid of cubic cells of
+// edge `edge` over the placed bounding box (one synchronisation); leaf: the cells are the leaves of a cloud
+int assess_place(Ctx* c, int as_run, const PoseD& cand, double edge, bool leaf, AsGrid& G, const double* lag = nullptr) {
     Ctx::Assess& A = c->A;
     const int n = (int)A.n;
     int box[8] = {0x7fffffff, 0x7fffffff, 0x7fffffff, -0x7fffffff - 1, -0x7fffffff - 1, -0x7fffffff - 1, 0, 0};
     CU(cudaMemcpyAsync(A.box, box, sizeof(box), cudaMemcpyHostToDevice, c->stream));
-    k_as_place<<<nblk(n, 256), 256, 0, c->stream>>>(A.pts, A.poses, n, as_run, cand, edge, A.world, A.box);
-    c->launches++;
+    if (lag) {
+        k_at_scan_end<<<nblk(A.scans, 128), 128, 0, c->stream>>>(A.at, A.pool, A.scans, *lag, as_run, cand, A.at_end);
+        k_at_place<<<nblk(n, 256), 256, 0, c->stream>>>(A.pts, A.raw, A.poses, A.at, A.at_end, A.pool, n, *lag, as_run, cand, edge, A.world, A.box);
+        c->launches += 2;
+    } else {
+        k_as_place<<<nblk(n, 256), 256, 0, c->stream>>>(A.pts, A.poses, n, as_run, cand, edge, A.world, A.box);
+        c->launches++;
+    }
     CU(cudaGetLastError());
     CU(cudaMemcpyAsync(box, A.box, sizeof(box), cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
@@ -2304,7 +2329,9 @@ PoseD assess_candidate(const liinit_assess_params* prm, const double* R_LI, cons
 // the cell edge of a radius: r (1 + 2^-20), see li_as_cell
 double assess_edge(double r) { return r * (1.0 + ldexp(1.0, -20)); }
 
-int assess_evaluate(Ctx* c, const liinit_assess_params* prm, const double* R_LI, const double* T_LI, liinit_assess_result* out) {
+// lag: a timed evaluation at that lag shift (assess_place)
+int assess_evaluate(Ctx* c, const liinit_assess_params* prm, const double* R_LI, const double* T_LI, liinit_assess_result* out,
+                    const double* lag = nullptr) {
     Ctx::Assess& A = c->A;
     const double r = prm->radius;
     int rc = assess_check_params(c, prm, R_LI, T_LI, false);
@@ -2316,7 +2343,7 @@ int assess_evaluate(Ctx* c, const liinit_assess_params* prm, const double* R_LI,
     if (nq > LIINIT_ASSESS_MAX_QUERIES)
         return fail(c, LIINIT_ERR_CAPACITY, "query_stride gives " + std::to_string(nq) + " queries, more than LIINIT_ASSESS_MAX_QUERIES");
     AsGrid G;
-    rc = assess_place(c, prm->as_run ? 1 : 0, assess_candidate(prm, R_LI, T_LI), assess_edge(r), false, G);
+    rc = assess_place(c, prm->as_run ? 1 : 0, assess_candidate(prm, R_LI, T_LI), assess_edge(r), false, G, lag);
     if (rc) return rc;
     int cur;
     rc = assess_sort(c, G, cur);
@@ -2495,9 +2522,12 @@ int assess_cloud(Ctx* c, const liinit_assess_params* prm, const double* R_LI, co
 
 extern "C" {
 
-int liinit_assess_reserve(liinit_ctx* h, long long max_points, int max_scans) {
-    if (!h) return LIINIT_ERR_INVALID;
-    Ctx* c = &h->c;
+}  // extern "C"
+
+namespace {
+
+// liinit_assess_reserve, and with max_pose_rows > 0 liinit_assess_reserve_timed
+int assess_reserve(Ctx* c, long long max_points, int max_scans, long long max_pose_rows) {
     if (has_comm(c)) return fail(c, LIINIT_ERR_INVALID, "the map assessment does not take a communicator (liinit_comm_init)");
     if (max_points < 1 || max_points > LIINIT_ASSESS_MAX_POINTS) return fail(c, LIINIT_ERR_INVALID, "max_points must be in [1, LIINIT_ASSESS_MAX_POINTS]");
     if (max_scans < 1 || max_scans > LIINIT_ASSESS_MAX_SCANS) return fail(c, LIINIT_ERR_INVALID, "max_scans must be in [1, LIINIT_ASSESS_MAX_SCANS]");
@@ -2517,6 +2547,10 @@ int liinit_assess_reserve(liinit_ctx* h, long long max_points, int max_scans) {
               cudaMalloc(&A.tasks, Q * sizeof(int4)) == cudaSuccess && cudaMalloc(&A.qn, Q * 4) == cudaSuccess && cudaMalloc(&A.qh, Q * 8) == cudaSuccess &&
               cudaMalloc(&A.qv, Q * 8) == cudaSuccess && cudaMalloc(&A.box, 8 * 4) == cudaSuccess && cudaMalloc(&A.tot, sizeof(AsTotals)) == cudaSuccess &&
               cudaMalloc(&A.ticket, sizeof(unsigned)) == cudaSuccess;
+    if (ok && max_pose_rows > 0)
+        ok = cudaMalloc(&A.raw, N * sizeof(float4)) == cudaSuccess && cudaMalloc(&A.at, (size_t)max_scans * sizeof(AtScan)) == cudaSuccess &&
+             cudaMalloc(&A.at_end, (size_t)max_scans * sizeof(PoseD)) == cudaSuccess &&
+             cudaMalloc(&A.pool, (size_t)max_pose_rows * LI_POSE6D_DOUBLES * sizeof(double)) == cudaSuccess;
     if (ok) A.k[1] = A.k[0] + N;   // one allocation: a cloud keeps n doubles in it (assess_cloud)
     if (!ok) {
         cudaGetLastError();
@@ -2525,7 +2559,46 @@ int liinit_assess_reserve(liinit_ctx* h, long long max_points, int max_scans) {
     }
     A.cap = max_points;
     A.max_scans = max_scans;
+    A.timed = max_pose_rows > 0;
+    A.pool_cap = max_pose_rows;
     return LIINIT_OK;
+}
+
+// the store of liinit_assess_append (k_as_store) for a staged cloud that fits; a timed store also records the scan's timing (timing
+// NULL: an untimed scan)
+int assess_store(Ctx* c, const double* rot_end, const double* pos_end, const double* R_LI, const double* T_LI, const AtScan* timing = nullptr) {
+    Ctx::Assess& A = c->A;
+    PoseD P;
+    fill_pose(P, rot_end, pos_end, R_LI, T_LI);
+    if (A.timed) {
+        const AtScan untimed{};   // npose = 0
+        CU(cudaMemcpyAsync(A.at + A.scans, timing ? timing : &untimed, sizeof(AtScan), cudaMemcpyHostToDevice, c->stream));
+        if (timing) A.timed_scans++; else A.untimed_scans++;
+    }
+    k_as_store<<<nblk(c->raw_n, 256), 256, 0, c->stream>>>(c->d_stage_pts, c->raw_n, A.scans, P, A.pts + A.n, A.poses);
+    c->launches++;
+    CU(cudaGetLastError());
+    A.n += c->raw_n;
+    A.scans++;
+    A.hold_seq = -1;
+    return LIINIT_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int liinit_assess_reserve(liinit_ctx* h, long long max_points, int max_scans) {
+    if (!h) return LIINIT_ERR_INVALID;
+    return assess_reserve(&h->c, max_points, max_scans, 0);
+}
+
+int liinit_assess_reserve_timed(liinit_ctx* h, long long max_points, int max_scans, long long max_pose_rows) {
+    if (!h) return LIINIT_ERR_INVALID;
+    Ctx* c = &h->c;
+    if (max_pose_rows < 2 || max_pose_rows > LIINIT_ASSESS_MAX_POSE_ROWS)
+        return fail(c, LIINIT_ERR_INVALID, "max_pose_rows must be in [2, LIINIT_ASSESS_MAX_POSE_ROWS]");
+    return assess_reserve(c, max_points, max_scans, max_pose_rows);
 }
 
 int liinit_assess_append(liinit_ctx* h, const double rot_end[9], const double pos_end[3], const double R_LI[9], const double T_LI[3],
@@ -2543,14 +2616,81 @@ int liinit_assess_append(liinit_ctx* h, const double rot_end[9], const double po
         *appended = 0;
         return LIINIT_OK;
     }
-    PoseD P;
-    fill_pose(P, rot_end, pos_end, R_LI, T_LI);
-    k_as_store<<<nblk(c->raw_n, 256), 256, 0, c->stream>>>(c->d_stage_pts, c->raw_n, A.scans, P, A.pts + A.n, A.poses);
-    c->launches++;
-    CU(cudaGetLastError());
-    A.n += c->raw_n;
-    A.scans++;
+    r = assess_store(c, rot_end, pos_end, R_LI, T_LI);
+    if (r) return r;
     *appended = 1;
+    return LIINIT_OK;
+}
+
+int liinit_assess_hold(liinit_ctx* h) {
+    if (!h) return LIINIT_ERR_INVALID;
+    Ctx* c = &h->c;
+    int r = assess_check(c);
+    if (r) return r;
+    Ctx::Assess& A = c->A;
+    if (!A.timed) return fail(c, LIINIT_ERR_INVALID, "the assessment store is not timed (liinit_assess_reserve_timed)");
+    if (c->raw_n <= 0) return fail(c, LIINIT_ERR_INVALID, "no raw cloud staged (liinit_raw_upload / liinit_frame_stage)");
+    CU(cudaSetDevice(c->device));
+    // a cloud the store has no room for is not copied: its append is skipped
+    if (A.n + c->raw_n <= A.cap)
+        CU(cudaMemcpyAsync(A.raw + A.n, c->d_stage_pts, (size_t)c->raw_n * sizeof(float4), cudaMemcpyDeviceToDevice, c->stream));
+    A.hold_seq = c->stage_seq;
+    A.hold_n = c->raw_n;
+    A.hold_at = A.n;
+    return LIINIT_OK;
+}
+
+int liinit_assess_append_timed(liinit_ctx* h, const double rot_end[9], const double pos_end[3], const double R_LI[9], const double T_LI[3],
+                               const liinit_assess_timing* t, int* appended) {
+    if (!h) return LIINIT_ERR_INVALID;
+    Ctx* c = &h->c;
+    if (!rot_end || !pos_end || !R_LI || !T_LI || !t || !appended) return fail(c, LIINIT_ERR_INVALID, "null argument");
+    int r = assess_check(c);
+    if (r) return r;
+    Ctx::Assess& A = c->A;
+    if (!A.timed) return fail(c, LIINIT_ERR_INVALID, "the assessment store is not timed (liinit_assess_reserve_timed)");
+    if (c->raw_n <= 0) return fail(c, LIINIT_ERR_INVALID, "no raw cloud staged (liinit_raw_upload / liinit_frame_stage)");
+    if (A.hold_seq != c->stage_seq || A.hold_at != A.n)
+        return fail(c, LIINIT_ERR_INVALID, "no hold of the staged cloud (liinit_assess_hold after staging it, before the undistortion)");
+    if (A.hold_n != c->raw_n) return fail(c, LIINIT_ERR_INVALID, "the held cloud and the staged cloud differ in size");
+    if (t->npose < 2 || t->npose > LIINIT_MAX_IMU_POSES) return fail(c, LIINIT_ERR_INVALID, "npose must be in [2, LIINIT_MAX_IMU_POSES]");
+    if (!t->poses) return fail(c, LIINIT_ERR_INVALID, "null pose table");
+    CU(cudaSetDevice(c->device));
+    if (A.n + c->raw_n > A.cap || A.scans >= A.max_scans) {
+        A.skipped++;
+        A.hold_seq = -1;
+        *appended = 0;
+        return LIINIT_OK;
+    }
+    if (A.pool_rows + t->npose > A.pool_cap) {   // no room for the table: stored as an untimed scan
+        r = assess_store(c, rot_end, pos_end, R_LI, T_LI);
+        if (r) return r;
+        *appended = 1;
+        return LIINIT_OK;
+    }
+    AtScan s{};
+    fill_pose(s.prior, t->rot, t->pos, t->R_LI, t->T_LI);
+    memcpy(s.vel, t->vel, 24);
+    s.row0 = A.pool_rows;
+    s.npose = t->npose;
+    CU(cudaMemcpyAsync(A.pool + (size_t)A.pool_rows * LI_POSE6D_DOUBLES, t->poses, (size_t)t->npose * LI_POSE6D_DOUBLES * sizeof(double),
+                       cudaMemcpyHostToDevice, c->stream));
+    A.pool_rows += t->npose;
+    r = assess_store(c, rot_end, pos_end, R_LI, T_LI, &s);
+    if (r) return r;
+    *appended = 1;
+    return LIINIT_OK;
+}
+
+int liinit_assess_timing_info(liinit_ctx* h, int* timed_scans, int* untimed_scans, long long* pose_rows) {
+    if (!h) return LIINIT_ERR_INVALID;
+    Ctx* c = &h->c;
+    int r = assess_check(c);
+    if (r) return r;
+    if (!c->A.timed) return fail(c, LIINIT_ERR_INVALID, "the assessment store is not timed (liinit_assess_reserve_timed)");
+    if (timed_scans) *timed_scans = c->A.timed_scans;
+    if (untimed_scans) *untimed_scans = c->A.untimed_scans;
+    if (pose_rows) *pose_rows = c->A.pool_rows;
     return LIINIT_OK;
 }
 
@@ -2573,6 +2713,19 @@ int liinit_assess_evaluate(liinit_ctx* h, const liinit_assess_params* p, const d
     if (r) return r;
     CU(cudaSetDevice(c->device));
     return assess_evaluate(c, p, R_LI, T_LI, out);
+}
+
+int liinit_assess_evaluate_timed(liinit_ctx* h, const liinit_assess_params* p, const double R_LI[9], const double T_LI[3], double lag_shift,
+                                 liinit_assess_result* out) {
+    if (!h) return LIINIT_ERR_INVALID;
+    Ctx* c = &h->c;
+    if (!p || !out) return fail(c, LIINIT_ERR_INVALID, "null argument");
+    int r = assess_check(c);
+    if (r) return r;
+    if (!c->A.timed) return fail(c, LIINIT_ERR_INVALID, "the assessment store is not timed (liinit_assess_reserve_timed)");
+    if (!std::isfinite(lag_shift)) return fail(c, LIINIT_ERR_INVALID, "lag_shift must be finite");
+    CU(cudaSetDevice(c->device));
+    return assess_evaluate(c, p, R_LI, T_LI, out, &lag_shift);
 }
 
 int liinit_assess_cloud(liinit_ctx* h, const liinit_assess_params* p, const double R_LI[9], const double T_LI[3], double leaf, float* rec8,

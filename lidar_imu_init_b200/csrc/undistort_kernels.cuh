@@ -62,17 +62,17 @@ __global__ void k_undistort_cv(float4* __restrict__ pts, int n, CvParams P, cons
 // Pose6D (msg/Pose6D.msg; common_lib.h:184-199), flat: offset_time, acc[3], gyr[3], vel[3], pos[3], rot[9] = 22 doubles
 #define LI_POSE6D_DOUBLES 22
 
-__global__ void k_undistort_imu(float4* __restrict__ pts, int n, const double* __restrict__ poses, int npose, PoseD S) {
-    int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    float4 p = pts[i];
-    const double t = (double)p.w / 1000.0;
-    // head = the last pose k <= npose-2 with offset_time < t
+// the head pose of a point at time t [s]: the last pose k <= npose-2 with offset_time < t (-1: none)
+__device__ __forceinline__ int li_imu_head(const double* __restrict__ poses, int npose, double t) {
     int head = -1;
     for (int k = 0; k <= npose - 2; k++)
         if (t > poses[(size_t)k * LI_POSE6D_DOUBLES]) head = k;
-    if (head < 0) return;
-    const double* h = poses + (size_t)head * LI_POSE6D_DOUBLES;
+    return head;
+}
+
+// the point (x, y, z) at time t [s] carried from the head pose h to the scan-end frame of S (rot_end, pos_end, R_LI, T_LI); shared by
+// k_undistort_imu and the timed assessment (assess_time_kernels.cuh), so both round alike
+__device__ __forceinline__ float3 li_undistort_imu_point(const double* __restrict__ h, double t, const PoseD& S, float px, float py, float pz) {
     const double dt = t - h[0];
     double E[9], Ri[9];
     li_so3_exp_dt(h + 4, dt, E);
@@ -84,7 +84,7 @@ __global__ void k_undistort_imu(float4* __restrict__ pts, int n, const double* _
     double Pi[3];
 #pragma unroll
     for (int a = 0; a < 3; a++) Pi[a] = h[10 + a] + h[7 + a] * dt + 0.5 * h[1 + a] * dt * dt;
-    const double x = p.x, y = p.y, z = p.z;
+    const double x = px, y = py, z = pz;
     double q[3], u[3], v[3], w[3];
 #pragma unroll
     for (int a = 0; a < 3; a++) q[a] = S.RLI[3 * a] * x + S.RLI[3 * a + 1] * y + S.RLI[3 * a + 2] * z + S.TLI[a];
@@ -94,7 +94,18 @@ __global__ void k_undistort_imu(float4* __restrict__ pts, int n, const double* _
     for (int a = 0; a < 3; a++) v[a] = S.R[a] * u[0] + S.R[3 + a] * u[1] + S.R[6 + a] * u[2] - S.TLI[a];   // rot_end^T u - T_LI
 #pragma unroll
     for (int a = 0; a < 3; a++) w[a] = S.RLI[a] * v[0] + S.RLI[3 + a] * v[1] + S.RLI[6 + a] * v[2];        // R_LI^T v
-    pts[i] = make_float4((float)w[0], (float)w[1], (float)w[2], p.w);
+    return make_float3((float)w[0], (float)w[1], (float)w[2]);
+}
+
+__global__ void k_undistort_imu(float4* __restrict__ pts, int n, const double* __restrict__ poses, int npose, PoseD S) {
+    int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    float4 p = pts[i];
+    const double t = (double)p.w / 1000.0;
+    const int head = li_imu_head(poses, npose, t);
+    if (head < 0) return;
+    const float3 w = li_undistort_imu_point(poses + (size_t)head * LI_POSE6D_DOUBLES, t, S, p.x, p.y, p.z);
+    pts[i] = make_float4(w.x, w.y, w.z, p.w);
 }
 
 // pointBodyToWorld (laserMapping.cpp:209-220) over the staged cloud, one thread per point, packed xyz out in upload order

@@ -308,7 +308,11 @@ class Node:
             self.recorder.update(t, pos, q, o.published)
         # (the switch scan re-filters the previous scan's cloud; LiDAR-only updates have no extrinsic in the model)
         if self.assess is not None and o.imu_en and o.switch_scan != o.frame_num - 1:
-            self.assess.append(R, p, RLI, TLI)
+            timing = getattr(o, "timing", None)
+            if getattr(self.assess, "timed", False) and timing is not None and len(timing[0]) >= 2:
+                self.assess.append_timed(R, p, RLI, TLI, *timing)   # the scan's raw cloud, pose table and propagated state
+            else:
+                self.assess.append(R, p, RLI, TLI)
         if self.on_update is not None:               # the posterior of the update, before the hand-over of a trigger scan
             self.on_update(self)
         # the refinement clock (:1169-1187)

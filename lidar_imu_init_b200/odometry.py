@@ -136,6 +136,10 @@ class LidarOdometry:
         self.scan_wait_num = 0
         self.pcd_index = 0
         self.pcd_files = []
+        # a timed assessment (assess.Assessment(timed=True)): the IMU undistortion holds the staged raw cloud for the store, and
+        # timing keeps (pose table, propagated state) of the last process_raw that undistorted from a table (None for any other)
+        self.assess_hold = False
+        self.timing = None
 
     def push_imu(self, omg, acc, t, mean_acc_norm=9.81):
         """imu_cbk in LO mode (:428-430)."""
@@ -192,6 +196,7 @@ class LidarOdometry:
         t_end = t_beg + end_ms / 1000.0                     # lidar_end_time (:455-456)
         group = self.imu_buffer.pop(t_end) if imu_group is None else np.asarray(imu_group, float).reshape(-1, 7)
         self.published = {}
+        self.timing = None
         if not self.imu_en:
             # Forward_propagation_without_imu (IMU_Processing.hpp:204-267)
             if self.first_prop:
@@ -205,6 +210,7 @@ class LidarOdometry:
         elif len(group) and not self.imu_proc.need_init:
             self.state, poses = self._propagate_imu(self.state, group, t_beg, end_ms)   # propagation_and_undist (:269-416)
             self._undistort_imu(raw, poses, self.state)
+            self.timing = (poses, self.state.copy())
         elif len(group):
             self.imu_proc.switch(group)                     # Process, IMU_Processing.hpp:445-453: no propagation, cloud kept
             self.switch_scan = self.frame_num
@@ -370,6 +376,8 @@ class LidarOdometry:
 
     def _undistort_imu(self, raw, poses, state):
         self._stage(raw)
+        if self.assess_hold:
+            self.g.assess_hold()
         if len(poses) >= 2:   # (one pose: the back-propagation loop of the reference runs zero times)
             R, p, RLI, TLI = host.state_pose(state)
             self.g.raw_undistort_imu(poses, R, p, RLI, TLI)

@@ -4,7 +4,7 @@
                                       [--max-map-points N] [--record PATH [--record-format ros1|ros2]
                                       [--record-compression none|bz2] [--record-topics a,b,...]] [--debug-logs]
                                       [--assess] [--assess-cloud PATH [--assess-cloud-leaf L]] [--assess-radius R]
-                                      [--assess-max-points N]
+                                      [--assess-max-points N] [--assess-time]
 
 --bag is a ROS1 bag (v2.0), a rosbag2 directory (sqlite3 storage) or one of its .db3 files, told apart by the file's first bytes. The
 LiDAR topic carries livox_ros_driver/CustomMsg or livox_ros_driver2/CustomMsg (lidar_type 1) or sensor_msgs/PointCloud2 in a ROS1
@@ -23,6 +23,8 @@ directory for a ROS 2 input, or as --record-format says. --debug-logs writes LI-
 map entropy and plane variance of the as-run, final and perturbed extrinsics, written to DIR/result/assessment.txt (assess).
 --assess-cloud PATH (with or without --assess) writes where the as-run map is blurred: the entropy and plane variance of every stored
 point, averaged over cubic leaves of --assess-cloud-leaf metres (0: every point), as a binary PCD.
+--assess-time also keeps each LIO scan's raw cloud and IMU pose table, re-undistorts the scans for every candidate, and scores the
+time lag too: the 14 candidates and a lag profile around the run's lag, written to DIR/result/assessment_time.txt.
 """
 from __future__ import annotations
 
@@ -68,6 +70,8 @@ def parse_args(argv=None):
                     help=f"leaf edge of --assess-cloud [m] (default {assessmod.CLOUD_LEAF:g}; 0: one record per stored point)")
     ap.add_argument("--assess-max-points", type=int, default=assessmod.MAX_POINTS, metavar="N",
                     help=f"LIO points the assessment stores on the device (default {assessmod.MAX_POINTS}); later scans are skipped")
+    ap.add_argument("--assess-time", action="store_true", help="score the time lag too, re-undistorting the stored LIO scans for every "
+                    "candidate: DIR/result/assessment_time.txt (stores the LIO scans like --assess)")
     return ap.parse_args(argv)
 
 
@@ -103,7 +107,7 @@ def main(argv=None, on_node=None) -> int:
     try:
         cfg = cfgmod.load(args.config, args.param)
         topics = record_topics(args)
-        assessing = args.assess or args.assess_cloud is not None
+        assessing = args.assess or args.assess_cloud is not None or args.assess_time
         if assessing and not (args.assess_radius > 0 and args.assess_radius < float("inf")):
             raise cfgmod.ConfigError(f"--assess-radius {args.assess_radius!r}: must be a positive number of metres")
         if args.assess_cloud is not None and not (args.assess_cloud_leaf >= 0 and args.assess_cloud_leaf < float("inf")):
@@ -122,7 +126,8 @@ def main(argv=None, on_node=None) -> int:
             if args.debug_logs:
                 node.open_debug_logs()
             if assessing:
-                node.assess = assessmod.Assessment(node.odom.g, args.assess_max_points, args.assess_radius)
+                node.assess = assessmod.Assessment(node.odom.g, args.assess_max_points, args.assess_radius, timed=args.assess_time)
+                node.odom.assess_hold = args.assess_time
             if on_node is not None:
                 on_node(node)
             t0 = time.perf_counter()
@@ -133,6 +138,11 @@ def main(argv=None, on_node=None) -> int:
             t0 = time.perf_counter()
             node.assess.write(os.path.join(args.out, "result", "assessment.txt"))
             log.info(f"assessment written to {os.path.join(args.out, 'result', 'assessment.txt')} in {time.perf_counter() - t0:.1f} s")
+        if args.assess_time:
+            t0 = time.perf_counter()
+            path = os.path.join(args.out, "result", "assessment_time.txt")
+            node.assess.write_time(path, node.time_lag)
+            log.info(f"time assessment written to {path} in {time.perf_counter() - t0:.1f} s")
         if args.assess_cloud is not None:
             t0 = time.perf_counter()
             got = node.assess.write_cloud(args.assess_cloud, args.assess_cloud_leaf)
