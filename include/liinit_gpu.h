@@ -423,6 +423,29 @@ int liinit_assess_timing_info(liinit_ctx* h, int* timed_scans, int* untimed_scan
  * LIINIT_ERR_INVALID for a store that is not timed or a non-finite lag_shift. */
 int liinit_assess_evaluate_timed(liinit_ctx* h, const liinit_assess_params* p, const double R_LI[9], const double T_LI[3], double lag_shift,
                                  liinit_assess_result* out);
+/* Empties the store (plain or timed) and keeps its reservation: no stored point, scan, skip, pose row or evaluation. */
+int liinit_assess_clear(liinit_ctx* h);
+
+/* LIO-phase replay (DESIGN.md section 4d): run the LIO loop again from the hand-over for a candidate calibration ------------------------
+ * liinit_map_snapshot copies the whole map state device to device on the context's stream: hash table, the used part of the brick list
+ * and of the point pool, the counters, the cell directory when there is one, and the staged raw cloud (the cloud the scan after the
+ * hand-over downsamples again). liinit_map_restore copies it back: every map entry point then behaves as it did at the snapshot, and the
+ * staged raw cloud is the snapshot's. The first snapshot allocates the hash-sized buffers; the pool and staging copies grow on demand.
+ * *bytes (may be NULL): bytes the snapshot copied. liinit_map_restore without a snapshot: LIINIT_ERR_INVALID. */
+int liinit_map_snapshot(liinit_ctx* h, long long* bytes);
+int liinit_map_restore(liinit_ctx* h);
+/* The replay store keeps sub-frames as liinit_frame_stage would stage them: xyz and time [ms] (16 bytes per point), intensity (4 bytes)
+ * and each sub-frame's lidar_beg_time and end offset [ms]. liinit_replay_reserve allocates it (again: clears it). */
+int liinit_replay_reserve(liinit_ctx* h, long long max_points, int max_frames);
+/* Copies sub-frame `handle` (liinit_frame_cut_*) into the store, device to device, with its t_beg [s] and end_ms. A sub-frame that does
+ * not fit is skipped and counted (*appended = 0). LIINIT_ERR_INVALID without a reserve or for an unknown handle. */
+int liinit_replay_append(liinit_ctx* h, long long handle, double t_beg, float end_ms, int* appended);
+/* Stored sub-frames, skipped ones and stored points (any pointer may be NULL). */
+int liinit_replay_info(liinit_ctx* h, int* frames, int* skipped, long long* points);
+/* t_beg, end_ms and point count of stored sub-frame j (any pointer may be NULL). */
+int liinit_replay_frame(liinit_ctx* h, int j, double* t_beg, float* end_ms, int* n);
+/* Stages stored sub-frame j as the raw cloud, exactly as liinit_frame_stage staged the original. */
+int liinit_replay_stage(liinit_ctx* h, int j);
 
 #ifdef __cplusplus
 }

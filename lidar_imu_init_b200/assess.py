@@ -18,6 +18,7 @@ shifts score a higher MME than the run's lag, `flat` otherwise.
 from __future__ import annotations
 
 import math
+from collections import deque
 
 import numpy as np
 
@@ -229,3 +230,230 @@ def parse_time_report(text: str) -> dict:
     f = ls[-1].split()
     assert f[0] == "lag" and f[2] == "best_shift_ms", ls[-1]
     return {"header": header, "assessment": rep, "profile": prof, "lag": (f[1], float(f[3]))}
+
+
+# ---- LIO-phase replay -----------------------------------------------------------------------------------------------------------------
+REPLAY_MAX_POINTS = 30_000_000   # raw LIO-phase points the replay store keeps on the device (20 bytes each)
+REPLAY_LAG_MS = 5.0              # lag shifts of the replay sweep [ms]
+
+
+class ReplayError(RuntimeError):
+    pass
+
+
+def _clone_odometry(odom):
+    """A copy of a LidarOdometry whose loop state can change without touching the original: the state, the IMU processor, the IMU buffer
+    and the per-scan bookkeeping are copied; the device context and the configuration are shared. It publishes nothing and feeds no
+    timed store."""
+    import copy
+    from collections import deque
+
+    from . import host
+    from .odometry import ImuBuffer
+    o = copy.copy(odom)
+    o.state = np.array(odom.state, float, copy=True)
+    o.imu_proc = copy.copy(odom.imu_proc)
+    o.imu_proc.m = host.Imu.from_buffer_copy(odom.imu_proc.m)
+    ib = ImuBuffer(odom.imu_buffer.timediff)
+    ib.time_lag, ib.last_stamp = odom.imu_buffer.time_lag, odom.imu_buffer.last_stamp
+    ib.rows = deque(np.array(r, float, copy=True) for r in odom.imu_buffer.rows)
+    o.imu_buffer = ib
+    o.preprocess = dict(odom.preprocess)
+    o.lidar_buffer = deque()
+    o.publish, o.published = None, {}
+    o.assess_hold, o.timing, o.replay = False, None, None
+    return o
+
+
+class Replay:
+    """Runs the LIO phase of a run again from the hand-over with a candidate calibration, and scores the map that run builds (DESIGN §4d).
+
+    During the run (Node.replay, LidarOdometry.replay): capture() takes the LiDAR-only odometry and the device map as LI-Init found them,
+    before the hand-over; after it, every sub-frame the loop processes goes to the device replay store (record_frame), every IMU sample
+    is kept in arrival order (record_imu) and every posterior state too (record_update). run() restores the map, hands over with the
+    candidate extrinsic and the candidate lag (LidarOdometry.hand_over on a copy of the captured odometry), and drives the same loop body
+    (process_raw, staging from the store) over the recorded input; the updates but the switch scan fill the plain assessment store, which
+    is then scored as run."""
+
+    def __init__(self, gpu, assessment: Assessment, max_points=REPLAY_MAX_POINTS, max_frames=MAX_SCANS):
+        self.g, self.assessment = gpu, assessment
+        self.g.replay_reserve(int(max_points), int(max_frames))
+        self.base = None          # the LidarOdometry before the hand-over (a copy)
+        self.res = None           # LI-Init's result
+        self.snapshot_bytes = 0
+        self.events = []          # after the hand-over, in arrival order: stored sub-frame index (int) or IMU sample (stamp, gyr, acc)
+        self.frames = 0
+        self.run_states = []      # (stored sub-frame index, posterior state) of the run's updates after the hand-over
+
+    # ---- recording ----
+    def capture(self, odom, res):
+        if self.base is not None:
+            raise ReplayError("the hand-over has been captured already")
+        self.snapshot_bytes = self.g.map_snapshot()
+        self.base = _clone_odometry(odom)
+        self.res = dict(res)
+
+    def record_imu(self, stamp, gyr, acc):
+        if self.base is not None:
+            self.events.append((float(stamp), np.array(gyr, float), np.array(acc, float)))
+
+    def record_frame(self, entry):
+        if self.base is not None and self.g.replay_append(entry["handle"], entry["t_beg"], entry["end_ms"]):
+            self.events.append(self.frames)
+            self.frames += 1
+
+    def record_update(self, state):
+        if self.base is not None and self.frames:
+            self.run_states.append((self.frames - 1, np.array(state, float, copy=True)))
+
+    def info(self) -> dict:
+        return self.g.replay_info()
+
+    # ---- replay ----
+    def run(self, R_LI=None, T_LI=None, lag_shift: float = 0.0, frozen: bool = True) -> dict:
+        """One replay. R_LI / T_LI: the candidate extrinsic (None: LI-Init's); lag_shift [s]: added to LI-Init's total lag; frozen: the
+        extrinsic is held constant by every update. Returns {"result": the as-run evaluation, "states": [(sub-frame index, posterior
+        state)], "R_LI", "T_LI": the extrinsic the replay ended with, "rms_m": RMS LiDAR position difference to the run's updates at the
+        same sub-frames, "seconds"}."""
+        import time
+
+        from .odometry import ReplayFrame
+        if self.base is None:
+            raise ReplayError("nothing to replay: the run did not reach the hand-over")
+        info = self.info()
+        if info["skipped"]:
+            raise ReplayError(f"the replay store is truncated ({info['skipped']} sub-frames skipped): raise its max_points")
+        t0 = time.perf_counter()
+        frames = [self.g.replay_frame(j) for j in range(info["frames"])]
+        res = dict(self.res)
+        if R_LI is not None:
+            res["R_LI"], res["T_LI"] = np.asarray(R_LI, float).reshape(3, 3), np.asarray(T_LI, float).reshape(3)
+        res["time_lag_2"] = float(res["time_lag_2"]) + float(lag_shift)
+        o = _clone_odometry(self.base)
+        self.g.map_restore()
+        o.hand_over(res)
+        if frozen:
+            o.frozen = True
+            cov = o.state[36:].reshape(24, 24)
+            cov[6:12, :] = 0.0
+            cov[:, 6:12] = 0.0
+            o.imu_proc.set_cov("R_LI_cov", 0.0)
+            o.imu_proc.set_cov("T_LI_cov", 0.0)
+        self.g.assess_clear()
+        states = []
+        pending = deque()
+        for ev in self.events:
+            if isinstance(ev, int):
+                pending.append(ev)
+            else:
+                o.imu_buffer.push(*ev)
+            # sync_packages: a sub-frame waits for an IMU stamp at or after its end
+            while pending:
+                f = frames[pending[0]]
+                t_end = f["t_beg"] + float(f["end_ms"]) / 1000.0
+                if not o.imu_buffer.rows or not o.imu_buffer.ready(t_end):
+                    break
+                j = pending.popleft()
+                frame_num = o.frame_num
+                o.process_raw(ReplayFrame(j, f["end_ms"], f["n"]), f["t_beg"], o.imu_buffer.pop(t_end))
+                if o.frame_num != frame_num:
+                    states.append((j, o.state.copy()))
+                    if o.switch_scan != o.frame_num - 1:
+                        R, p, rli, tli = host_pose(o.state)
+                        self.g.assess_append(R, p, rli, tli)
+        a = self.assessment
+        result = self.g.assess_evaluate(radius=a.radius, min_neighbors=a.min_neighbors, as_run=True)
+        _, _, rli, tli = host_pose(o.state)
+        return dict(result=result, states=states, R_LI=rli, T_LI=tli, rms_m=trajectory_rms(self.run_states, states),
+                    seconds=time.perf_counter() - t0)
+
+    def sweep(self, R_final, T_final, dtheta_deg=DTHETA_DEG, dt=DT_M, lag_ms=REPLAY_LAG_MS) -> list:
+        """[(name, R_LI, T_LI, shift_ms, replay)] of the 17 replays: the run itself (not frozen), LI-Init's result, the final extrinsic,
+        its 12 perturbations, and the final extrinsic at lag shifts of -+lag_ms; all frozen but the first."""
+        R_init = np.asarray(self.res["R_LI"], float).reshape(3, 3)
+        T_init = np.asarray(self.res["T_LI"], float).reshape(3)
+        plan = [("run", R_init, T_init, 0.0, False), ("li-init", R_init, T_init, 0.0, True)]
+        plan += [(name, R, T, 0.0, True) for name, R, T in candidates(R_final, T_final, dtheta_deg, dt)[1:]]
+        plan += [(f"lag{s:+g}", plan[2][1], plan[2][2], s, True) for s in (-lag_ms, lag_ms)]
+        out = []
+        for name, R, T, shift_ms, frozen in plan:
+            r = self.run(None if name == "run" else R, None if name == "run" else T, shift_ms / 1000.0, frozen)
+            out.append((name, R, T, shift_ms, r))
+        return out
+
+    def report(self, R_final, T_final) -> str:
+        import time
+        t0 = time.perf_counter()
+        rows = self.sweep(R_final, T_final)
+        wall = time.perf_counter() - t0
+        return replay_report_text(self.info(), self.snapshot_bytes, wall, self.assessment.radius, self.assessment.min_neighbors, rows)
+
+    def write(self, path: str, R_final=None, T_final=None):
+        """result/assessment_replay.txt; R_final / T_final: the run's final extrinsic. NOTHING when the run did not hand over."""
+        with open(path, "w") as f:
+            f.write(NOTHING if self.base is None or not self.frames else self.report(R_final, T_final))
+
+
+def host_pose(state):
+    from . import host
+    return host.state_pose(state)
+
+
+def trajectory_rms(run_states, states) -> float:
+    """RMS difference [m] of the LiDAR positions (R T_LI + p) of two lists of (sub-frame index, state), over the indices both have."""
+    def lidar(s):
+        R, p, _, tli = host_pose(s)
+        return R @ tli + p
+    a = dict(run_states)
+    d = [lidar(s) - lidar(a[j]) for j, s in states if j in a]
+    return float(np.sqrt(np.mean(np.sum(np.square(d), axis=1)))) if d else float("nan")
+
+
+def replay_report_text(info: dict, snapshot_bytes: int, wall_s: float, radius: float, min_neighbors: int, rows: list, dtheta_deg=DTHETA_DEG,
+                       dt=DT_M) -> str:
+    """result/assessment_replay.txt: a header line of key value pairs, a column line, one fixed-column row per replay (the candidate, its
+    lag shift, the as-run score of the map the replay built, the extrinsic it ended with and the RMS LiDAR position difference to the run),
+    one line per axis and the lag line."""
+    from .node import rot_to_euler
+    lines = [f"subframes {info['frames']} skipped {info['skipped']} points {info['points']} snapshot_mb {snapshot_bytes / 1e6:.6f} "
+             f"replay_s {wall_s:.6f} radius {radius:.6f} n_min {min_neighbors} dtheta_deg {dtheta_deg:.6f} dt_m {dt:.6f}",
+             "%-9s %11s %11s %11s %10s %10s %10s %9s %10s %10s %10s %15s %15s %11s %11s %11s %10s %10s %10s %12s" % (
+                 "candidate", "roll_deg", "pitch_deg", "yaw_deg", "t_x", "t_y", "t_z", "shift_ms", "valid", "sparse", "degenerate", "mme",
+                 "mpv", "end_roll", "end_pitch", "end_yaw", "end_t_x", "end_t_y", "end_t_z", "rms_m")]
+    for name, R, T, shift_ms, r in rows:
+        e, ee, res, te = np.degrees(rot_to_euler(R)), np.degrees(rot_to_euler(r["R_LI"])), r["result"], r["T_LI"]
+        lines.append("%-9s %11.6f %11.6f %11.6f %10.6f %10.6f %10.6f %9.3f %10d %10d %10d %15.9f %15.9e %11.6f %11.6f %11.6f %10.6f %10.6f %10.6f "
+                     "%12.6e" % (name, e[0], e[1], e[2], T[0], T[1], T[2], shift_ms, res["valid"], res["sparse"], res["degenerate"], res["mme"],
+                                 res["mpv"], ee[0], ee[1], ee[2], te[0], te[1], te[2], r["rms_m"]))
+    by_name = {name: r["result"] for name, _, _, _, r in rows}
+    for axis, (v, dp, dm) in verdicts(by_name).items():
+        lines.append("%-7s %-11s %15.9f %15.9f" % (axis, v, dp, dm))
+    prof = [(s, r["result"]) for name, _, _, s, r in rows if name.startswith("lag")]
+    prof = sorted(prof + [(0.0, by_name["final"])], key=lambda x: x[0])
+    v, best = lag_verdict(prof)
+    m = {s: r["mme"] for s, r in prof}
+    lines.append(f"lag {v} best_shift_ms {best:.3f} d_minus {m[prof[0][0]] - m[0.0]:.9f} d_plus {m[prof[-1][0]] - m[0.0]:.9f}")
+    return "\n".join(lines) + "\n"
+
+
+def parse_replay_report(text: str) -> dict:
+    """The inverse of replay_report_text: {"header": {...}, "rows": {name: {...}}, "axes": {axis: (verdict, d_plus, d_minus)},
+    "lag": (verdict, best shift [ms], d_minus, d_plus)}, or {"nothing": True}."""
+    if text == NOTHING:
+        return {"nothing": True}
+    ls = text.splitlines()
+    h = ls[0].split()
+    header = {h[i]: float(h[i + 1]) if "." in h[i + 1] else int(h[i + 1]) for i in range(0, len(h), 2)}
+    cols = ls[1].split()
+    rows, axes = {}, {}
+    i = 2
+    while i < len(ls) and len(ls[i].split()) == len(cols):
+        f = ls[i].split()
+        rows[f[0]] = {c: (int(x) if c in ("valid", "sparse", "degenerate") else float(x)) for c, x in zip(cols[1:], f[1:])}
+        i += 1
+    for line in ls[i:-1]:
+        f = line.split()
+        axes[f[0]] = (f[1], float(f[2]), float(f[3]))
+    f = ls[-1].split()
+    assert f[0] == "lag" and f[2] == "best_shift_ms" and f[4] == "d_minus" and f[6] == "d_plus", ls[-1]
+    return {"header": header, "rows": rows, "axes": axes, "lag": (f[1], float(f[3]), float(f[5]), float(f[7]))}

@@ -94,7 +94,8 @@ SYMBOLS = [
     "liinit_map_nearest_search_device", "liinit_cloud_download_device", "liinit_map_download_device",
     "liinit_assess_reserve", "liinit_assess_append", "liinit_assess_info", "liinit_assess_evaluate", "liinit_assess_download",
     "liinit_assess_download_placed", "liinit_assess_cloud", "liinit_assess_reserve_timed", "liinit_assess_hold", "liinit_assess_append_timed",
-    "liinit_assess_timing_info", "liinit_assess_evaluate_timed",
+    "liinit_assess_timing_info", "liinit_assess_evaluate_timed", "liinit_assess_clear", "liinit_map_snapshot", "liinit_map_restore",
+    "liinit_replay_reserve", "liinit_replay_append", "liinit_replay_info", "liinit_replay_frame", "liinit_replay_stage",
 ]
 
 
@@ -194,6 +195,23 @@ def set_assess_argtypes(L):
     for s in ("reserve", "append", "info", "evaluate", "download", "download_placed", "cloud", "reserve_timed", "hold", "append_timed",
               "timing_info", "evaluate_timed"):
         getattr(L, "liinit_assess_" + s).restype = C.c_int
+    set_replay_argtypes(L)
+
+
+def set_replay_argtypes(L):
+    """argtypes of the LIO-phase replay entry points (liinit_assess_clear, liinit_map_snapshot / _restore, liinit_replay_*)"""
+    vp = C.c_void_p
+    L.liinit_assess_clear.argtypes = [vp]
+    L.liinit_map_snapshot.argtypes = [vp, C.POINTER(C.c_longlong)]
+    L.liinit_map_restore.argtypes = [vp]
+    L.liinit_replay_reserve.argtypes = [vp, C.c_longlong, C.c_int]
+    L.liinit_replay_append.argtypes = [vp, C.c_longlong, C.c_double, C.c_float, C.POINTER(C.c_int)]
+    L.liinit_replay_info.argtypes = [vp, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_longlong)]
+    L.liinit_replay_frame.argtypes = [vp, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_float), C.POINTER(C.c_int)]
+    L.liinit_replay_stage.argtypes = [vp, C.c_int]
+    for s in ("liinit_assess_clear", "liinit_map_snapshot", "liinit_map_restore", "liinit_replay_reserve", "liinit_replay_append",
+              "liinit_replay_info", "liinit_replay_frame", "liinit_replay_stage"):
+        getattr(L, s).restype = C.c_int
 
 
 def _pts(a):
@@ -737,6 +755,49 @@ class LiInitGpu:
         out = AssessResult()
         self._ck(self.L.liinit_assess_evaluate_timed(self.h, C.byref(P), _ptr(R), _ptr(T), float(lag_shift), C.byref(out)))
         return {k: getattr(out, k) for k, _ in AssessResult._fields_}
+
+    def assess_clear(self):
+        """Empty the assessment store, keeping its reservation."""
+        self._ck(self.L.liinit_assess_clear(self.h))
+
+    # ---- LIO-phase replay (DESIGN §4d) ----
+    def map_snapshot(self) -> int:
+        """Copy the map state and the staged raw cloud on the device; returns the bytes copied."""
+        b = C.c_longlong(0)
+        self._ck(self.L.liinit_map_snapshot(self.h, C.byref(b)))
+        self._snap_raw_n = getattr(self, "raw_n", 0)
+        return b.value
+
+    def map_restore(self):
+        """Put the map and the staged raw cloud back as map_snapshot found them."""
+        self._ck(self.L.liinit_map_restore(self.h))
+        self.raw_n = self._snap_raw_n
+
+    def replay_reserve(self, max_points: int, max_frames: int):
+        """Allocate (or clear) the store of the LIO phase's sub-frames."""
+        self._ck(self.L.liinit_replay_reserve(self.h, int(max_points), int(max_frames)))
+
+    def replay_append(self, handle: int, t_beg: float, end_ms) -> bool:
+        """Keep sub-frame `handle` with its lidar_beg_time and end offset [ms]; False when the store had no room (counted as skipped)."""
+        ok = C.c_int(0)
+        self._ck(self.L.liinit_replay_append(self.h, int(handle), float(t_beg), float(np.float32(end_ms)), C.byref(ok)))
+        return bool(ok.value)
+
+    def replay_info(self) -> dict:
+        f, k, p = C.c_int(0), C.c_int(0), C.c_longlong(0)
+        self._ck(self.L.liinit_replay_info(self.h, C.byref(f), C.byref(k), C.byref(p)))
+        return dict(frames=f.value, skipped=k.value, points=p.value)
+
+    def replay_frame(self, j: int) -> dict:
+        """{t_beg, end_ms (float32), n} of stored sub-frame j."""
+        t, e, n = C.c_double(0), C.c_float(0), C.c_int(0)
+        self._ck(self.L.liinit_replay_frame(self.h, int(j), C.byref(t), C.byref(e), C.byref(n)))
+        return dict(t_beg=t.value, end_ms=np.float32(e.value), n=n.value)
+
+    def replay_stage(self, j: int):
+        """Stored sub-frame j becomes the staged raw cloud, as frame_stage left the original."""
+        self._ck(self.L.liinit_replay_stage(self.h, int(j)))
+        self.raw_n = self.replay_frame(j)["n"]
 
     def knn_index(self) -> int:
         """1 = LIINIT_KNN_BRICKS (lockstep groups over whole bricks), 2 = LIINIT_KNN_CELLS (cell directory, thread per point)."""

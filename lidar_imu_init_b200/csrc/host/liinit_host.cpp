@@ -174,14 +174,80 @@ int liinit_ieskf_update(liinit_state* st, const liinit_state* prop, const double
     return ieskf_update(st, prop, HtH, Htr, sol, KH, nullptr);
 }
 
-int liinit_scan_update(liinit_ctx* h, liinit_state* state, int max_iter, int imu_en, liinit_scan_stats* stats) {
+// ---- the update with a constant extrinsic: the 18 states other than R_LI (6:9) and T_LI (9:12) ----
+constexpr int DF = D - 6;
+static const int kFree[DF] = {0, 1, 2, 3, 4, 5, 12, 13, 14, 15, 16, 17, 18, 19, 20, 21, 22, 23};
+
+// cov restricted to the free states, inverted (DF x DF)
+static bool free_cov_inverse(const double* P, double* out) {
+    double Pr[DF * DF];
+    for (int r = 0; r < DF; r++)
+        for (int c = 0; c < DF; c++) Pr[r * DF + c] = P[kFree[r] * D + kFree[c]];
+    return invert(Pr, out, DF);
+}
+
+static void zero_extrinsic_cov(double* P) {
+    for (int i = 6; i < 12; i++)
+        for (int j = 0; j < D; j++) P[i * D + j] = P[j * D + i] = 0.0;
+}
+
+// ieskf_update on the free states: K_1 = (blkdiag(1000 HtH[0:6,0:6], 0) + cov_r^-1)^-1, solution_r = K_1[:,0:6] (1000 Htr[0:6]) + vec_r -
+// K_1[:,0:6] (1000 HtH[0:6,0:6]) vec[0:6]; the extrinsic keeps its bits (Exp(0) and + 0 could still flip the sign of a zero)
+static int ieskf_update_frozen(liinit_state* st, const liinit_state* prop, const double* HtH, const double* Htr, double* sol, double* KH,
+                               const double* cov_inv_r) {
+    double S[DF * DF], K1[DF * DF];
+    if (cov_inv_r) std::memcpy(S, cov_inv_r, sizeof(S));
+    else if (!free_cov_inverse(st->cov, S)) return LIINIT_ERR_INVALID;
+    for (int a = 0; a < 6; a++)
+        for (int b = 0; b < 6; b++) S[a * DF + b] += 1000.0 * HtH[a * 12 + b];
+    if (!invert(S, K1, DF, 6)) return LIINIT_ERR_INVALID;
+    double vec[D], vr[DF];
+    liinit_state_boxminus(prop, st, vec);
+    for (int i = 0; i < DF; i++) vr[i] = vec[kFree[i]];
+    double G[DF * 6];
+    for (int r = 0; r < DF; r++)
+        for (int c = 0; c < 6; c++) {
+            double s = 0;
+            for (int a = 0; a < 6; a++) s += K1[r * DF + a] * (1000.0 * HtH[a * 12 + c]);
+            G[r * 6 + c] = s;
+        }
+    for (int i = 0; i < D; i++) sol[i] = 0.0;
+    for (int r = 0; r < DF; r++) {
+        double s = 0, t = 0;
+        for (int a = 0; a < 6; a++) {
+            s += K1[r * DF + a] * (1000.0 * Htr[a]);
+            t += G[r * 6 + a] * vr[a];
+        }
+        sol[kFree[r]] = s + vr[r] - t;
+    }
+    double RLI[9], TLI[3];
+    std::memcpy(RLI, st->offset_R_L_I, sizeof(RLI));
+    std::memcpy(TLI, st->offset_T_L_I, sizeof(TLI));
+    liinit_state_boxplus(st, sol);
+    std::memcpy(st->offset_R_L_I, RLI, sizeof(RLI));
+    std::memcpy(st->offset_T_L_I, TLI, sizeof(TLI));
+    if (KH) {
+        for (int i = 0; i < D * 12; i++) KH[i] = 0.0;
+        for (int r = 0; r < DF; r++)
+            for (int c = 0; c < 6; c++) KH[kFree[r] * 12 + c] = G[r * 6 + c];
+    }
+    zero_extrinsic_cov(st->cov);
+    return LIINIT_OK;
+}
+
+int liinit_ieskf_update_frozen(liinit_state* st, const liinit_state* prop, const double* HtH, const double* Htr, double* sol, double* KH) {
+    return ieskf_update_frozen(st, prop, HtH, Htr, sol, KH, nullptr);
+}
+
+static int scan_update(liinit_ctx* h, liinit_state* state, int max_iter, int imu_en, liinit_scan_stats* stats, bool frozen) {
     if (!h || !state || max_iter < 1) return LIINIT_ERR_INVALID;
     liinit_state prop = *state;            // state_propagat = state (laserMapping.cpp:910)
     int rematch_num = 0, nearest_search_en = 1;
     liinit_scan_stats st{};
     double HtH[144], Htr[12], sol[D], KH[D * 12];
     double cov_inv[D * D];                 // state.cov is only replaced at the end of the scan (:1127): one inversion for all iterations
-    if (!invert(state->cov, cov_inv, D)) return LIINIT_ERR_INVALID;
+    if (!(frozen ? free_cov_inverse(state->cov, cov_inv) : invert(state->cov, cov_inv, D))) return LIINIT_ERR_INVALID;
+    if (frozen) zero_extrinsic_cov(state->cov);
     for (int it = 0; it < max_iter; it++) {
         int m = 0;
         double rs = 0;
@@ -189,7 +255,7 @@ int liinit_scan_update(liinit_ctx* h, liinit_state* state, int max_iter, int imu
         int rc = liinit_icp_iterate(h, state->rot_end, state->pos_end, state->offset_R_L_I, state->offset_T_L_I, imu_en,
                                     nearest_search_en, HtH, Htr, &m, &rs);
         if (rc != LIINIT_OK) return rc;
-        rc = ieskf_update(state, &prop, HtH, Htr, sol, KH, cov_inv);
+        rc = frozen ? ieskf_update_frozen(state, &prop, HtH, Htr, sol, KH, cov_inv) : ieskf_update(state, &prop, HtH, Htr, sol, KH, cov_inv);
         if (rc != LIINIT_OK) return rc;
         st.iterations++;
         st.effect_feat_num = m;
@@ -219,6 +285,14 @@ int liinit_scan_update(liinit_ctx* h, liinit_state* state, int max_iter, int imu
     }
     if (stats) *stats = st;
     return LIINIT_OK;
+}
+
+int liinit_scan_update(liinit_ctx* h, liinit_state* state, int max_iter, int imu_en, liinit_scan_stats* stats) {
+    return scan_update(h, state, max_iter, imu_en, stats, false);
+}
+
+int liinit_scan_update_frozen(liinit_ctx* h, liinit_state* state, int max_iter, int imu_en, liinit_scan_stats* stats) {
+    return scan_update(h, state, max_iter, imu_en, stats, true);
 }
 
 // Exp(ang_vel, dt) (so3_math.h:39-59): gated on the angular VELOCITY (|w| > 1e-7), not on the angle like Exp(v1, v2, v3) (:61-80,

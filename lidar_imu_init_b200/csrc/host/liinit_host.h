@@ -59,6 +59,15 @@ int liinit_ieskf_update(liinit_state* state, const liinit_state* state_propagat,
  * state: in = propagated prior (state_propagat = state, :910), out = posterior. */
 int liinit_scan_update(liinit_ctx* h, liinit_state* state, int max_iteration, int imu_en, liinit_scan_stats* stats);
 
+/* liinit_ieskf_update and liinit_scan_update with the extrinsic (offset_R_L_I, offset_T_L_I: states 6:12) held constant, for a replay
+ * of the LIO phase with a candidate calibration. The update solves on the other 18 states: cov restricted to them is inverted, only the
+ * pose block HtH[0:6, 0:6] / Htr[0:6] of the 12-column Jacobian enters, and solution[6:12] = 0. The extrinsic is left bit for bit as it
+ * was, and on return its rows and columns of cov are zero (so are those of KH). With the extrinsic's propagation noise set to zero
+ * (liinit_imu_set_R_LI_cov / _T_LI_cov), liinit_imu_propagate keeps them zero. */
+int liinit_ieskf_update_frozen(liinit_state* state, const liinit_state* state_propagat, const double HtH[144], const double Htr[12],
+                               double solution[LIINIT_DIM_STATE], double* KH);
+int liinit_scan_update_frozen(liinit_ctx* h, liinit_state* state, int max_iteration, int imu_en, liinit_scan_stats* stats);
+
 /* State propagation of the LiDAR-only (constant-velocity) mode, ImuProcess::Forward_propagation_without_imu without its
  * point loop (src/IMU_Processing.hpp:212-243; the loop :246-266 is liinit_raw_undistort_cv): bias_g stands for the
  * angular velocity, vel_end for the linear velocity. cov <- F cov F^T + Q with F[0:3,0:3] = Exp(-bias_g dt),

@@ -248,6 +248,42 @@ struct Ctx {
         int hold_n = 0;            // ... its points ...
         long long hold_at = 0;     // ... and the stored-point count it was copied behind
     } A;
+    // LIO-phase replay (liinit_replay_*): sub-frames in the layout of the frame slots, appended in processing order
+    struct ReplayFrame {
+        double t_beg;
+        float end_ms;
+        int n;
+        long long lo;   // first stored point
+    };
+    struct Replay {
+        long long cap = 0, n = 0;   // points (cap 0: not reserved)
+        int max_frames = 0, skipped = 0;
+        float4* pts = nullptr;      // xyz, w = time [ms]
+        float* inten = nullptr;
+        std::vector<ReplayFrame> fr;
+    } R;
+    // map snapshot (liinit_map_snapshot / _restore): device copies of the map state and of the staged raw cloud, host copies of the
+    // counters the host mirrors
+    struct Snap {
+        bool have = false;
+        uint4* ent = nullptr;
+        uint4* aux = nullptr;
+        int* brick_slots = nullptr;
+        unsigned long long* cocc = nullptr;
+        unsigned short* cdir = nullptr;
+        unsigned long long* sb_keys = nullptr;
+        unsigned long long* sb_occ = nullptr;
+        int* counters = nullptr;                // CNT_COUNT ints, then the pool top as one 8-byte word
+        float4* pool = nullptr;
+        unsigned long long pool_alloc = 0;      // points
+        float4* stage_pts = nullptr;
+        float4* stage_attr = nullptr;
+        int stage_alloc = 0;                    // points
+        int h_counters[CNT_COUNT] = {};
+        unsigned long long pool_top = 0;
+        int raw_n = 0;
+        bool stage_attr_on = false;
+    } snap;
 };
 
 #define CU(call)                                                                                     \
@@ -826,6 +862,18 @@ void assess_free(Ctx* c) {
     A = Ctx::Assess{};
 }
 
+void replay_free(Ctx* c) {
+    cudaFree(c->R.pts); cudaFree(c->R.inten);
+    c->R = Ctx::Replay{};
+}
+
+void snap_free(Ctx* c) {
+    Ctx::Snap& S = c->snap;
+    cudaFree(S.ent); cudaFree(S.aux); cudaFree(S.brick_slots); cudaFree(S.cocc); cudaFree(S.cdir); cudaFree(S.sb_keys); cudaFree(S.sb_occ);
+    cudaFree(S.counters); cudaFree(S.pool); cudaFree(S.stage_pts); cudaFree(S.stage_attr);
+    S = Ctx::Snap{};
+}
+
 }  // namespace
 
 struct liinit_ctx {
@@ -1050,6 +1098,8 @@ int liinit_destroy(liinit_ctx* h) {
     cudaFree(c->d_partials); cudaFree(c->d_done); cudaFreeHost(c->h_out); cudaFree(c->d_q_d2);
     frame_free(c);
     assess_free(c);
+    replay_free(c);
+    snap_free(c);
     if (c->ev0) cudaEventDestroy(c->ev0);
     if (c->ev1) cudaEventDestroy(c->ev1);
     if (c->evm) cudaEventDestroy(c->evm);
@@ -2770,6 +2820,222 @@ int liinit_assess_download_placed(liinit_ctx* h, float* xyz, long long cap, long
     if (cap < m) return fail(c, LIINIT_ERR_CAPACITY, "cap is smaller than the number of stored points");
     CU(cudaSetDevice(c->device));
     return download_xyz(c, c->A.world, (size_t)m, xyz);
+}
+
+}  // extern "C"
+
+namespace {
+
+// cudaMalloc that first frees what p held (a snapshot buffer that has to grow)
+template <class T>
+cudaError_t regrow(T*& p, size_t count) {
+    cudaFree(p);
+    p = nullptr;
+    return cudaMalloc(&p, count * sizeof(T));
+}
+
+int map_snapshot(Ctx* c, long long* bytes) {
+    int r = fetch_counters(c);   // (synchronises: the host mirrors and the counts that size the copies are current)
+    if (r) return r;
+    Ctx::Snap& S = c->snap;
+    const size_t slots = c->hash_slots;
+    const unsigned long long top = *c->h_pool_top;
+    const int bricks = c->h_counters[CNT_BRICKS];
+    bool ok = true;
+    if (!S.ent) {
+        ok = cudaMalloc(&S.ent, slots * sizeof(uint4)) == cudaSuccess && cudaMalloc(&S.aux, slots * sizeof(uint4)) == cudaSuccess &&
+             cudaMalloc(&S.brick_slots, slots * sizeof(int)) == cudaSuccess &&
+             cudaMalloc(&S.counters, CNT_COUNT * sizeof(int) + sizeof(unsigned long long)) == cudaSuccess;
+        if (ok && c->cells)
+            ok = cudaMalloc(&S.cocc, slots * 8) == cudaSuccess && cudaMalloc(&S.cdir, slots * 64 * sizeof(unsigned short)) == cudaSuccess &&
+                 cudaMalloc(&S.sb_keys, slots * 8) == cudaSuccess && cudaMalloc(&S.sb_occ, slots * 8) == cudaSuccess;
+    }
+    if (ok && top > S.pool_alloc) {
+        ok = regrow(S.pool, (size_t)top) == cudaSuccess;
+        S.pool_alloc = ok ? top : 0;
+    }
+    if (ok && c->raw_n > S.stage_alloc) {
+        ok = regrow(S.stage_pts, (size_t)c->raw_n) == cudaSuccess && regrow(S.stage_attr, (size_t)c->raw_n) == cudaSuccess;
+        S.stage_alloc = ok ? c->raw_n : 0;
+    }
+    if (!ok) {
+        cudaGetLastError();
+        snap_free(c);
+        return fail(c, LIINIT_ERR_CUDA, "cudaMalloc of the map snapshot failed");
+    }
+    long long b = 0;
+    auto d2d = [&](void* dst, const void* src, size_t n) {
+        b += (long long)n;
+        return n ? cudaMemcpyAsync(dst, src, n, cudaMemcpyDeviceToDevice, c->stream) : cudaSuccess;
+    };
+    CU(d2d(S.ent, c->M.ent, slots * sizeof(uint4)));
+    CU(d2d(S.aux, c->M.aux, slots * sizeof(uint4)));
+    CU(d2d(S.brick_slots, c->M.brick_slots, (size_t)bricks * sizeof(int)));
+    CU(d2d(S.counters, c->d_counters, CNT_COUNT * sizeof(int)));
+    CU(d2d(S.counters + CNT_COUNT, c->M.pool_top, sizeof(unsigned long long)));
+    CU(d2d(S.pool, c->M.pool, (size_t)top * sizeof(float4)));
+    if (c->cells) {
+        CU(d2d(S.cocc, c->M.cocc, slots * 8));
+        CU(d2d(S.cdir, c->M.cdir, slots * 64 * sizeof(unsigned short)));
+        CU(d2d(S.sb_keys, c->M.sb_keys, slots * 8));
+        CU(d2d(S.sb_occ, c->M.sb_occ, slots * 8));
+    }
+    CU(d2d(S.stage_pts, c->d_stage_pts, (size_t)c->raw_n * sizeof(float4)));
+    if (c->stage_attr) CU(d2d(S.stage_attr, c->d_stage_attr, (size_t)c->raw_n * sizeof(float4)));
+    memcpy(S.h_counters, c->h_counters, sizeof(S.h_counters));
+    S.pool_top = top;
+    S.raw_n = c->raw_n;
+    S.stage_attr_on = c->stage_attr;
+    S.have = true;
+    if (bytes) *bytes = b;
+    return LIINIT_OK;
+}
+
+int map_restore(Ctx* c) {
+    Ctx::Snap& S = c->snap;
+    if (!S.have) return fail(c, LIINIT_ERR_INVALID, "no map snapshot (liinit_map_snapshot)");
+    const size_t slots = c->hash_slots;
+    auto d2d = [&](void* dst, const void* src, size_t n) {
+        return n ? cudaMemcpyAsync(dst, src, n, cudaMemcpyDeviceToDevice, c->stream) : cudaSuccess;
+    };
+    CU(d2d(c->M.ent, S.ent, slots * sizeof(uint4)));
+    CU(d2d(c->M.aux, S.aux, slots * sizeof(uint4)));
+    CU(d2d(c->M.brick_slots, S.brick_slots, (size_t)S.h_counters[CNT_BRICKS] * sizeof(int)));
+    CU(d2d(c->d_counters, S.counters, CNT_COUNT * sizeof(int)));
+    CU(d2d(c->M.pool_top, S.counters + CNT_COUNT, sizeof(unsigned long long)));
+    CU(d2d(c->M.pool, S.pool, (size_t)S.pool_top * sizeof(float4)));
+    if (c->cells) {
+        CU(d2d(c->M.cocc, S.cocc, slots * 8));
+        CU(d2d(c->M.cdir, S.cdir, slots * 64 * sizeof(unsigned short)));
+        CU(d2d(c->M.sb_keys, S.sb_keys, slots * 8));
+        CU(d2d(c->M.sb_occ, S.sb_occ, slots * 8));
+    }
+    CU(d2d(c->d_stage_pts, S.stage_pts, (size_t)S.raw_n * sizeof(float4)));
+    if (S.stage_attr_on) CU(d2d(c->d_stage_attr, S.stage_attr, (size_t)S.raw_n * sizeof(float4)));
+    memcpy(c->h_counters, S.h_counters, sizeof(S.h_counters));
+    *c->h_pool_top = S.pool_top;
+    c->map_epoch++;   // the restore can remove map points
+    c->raw_n = S.raw_n;
+    c->stage_attr = S.stage_attr_on;
+    c->stage_seq++;
+    return LIINIT_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int liinit_assess_clear(liinit_ctx* h) {
+    if (!h) return LIINIT_ERR_INVALID;
+    Ctx* c = &h->c;
+    int r = assess_check(c);
+    if (r) return r;
+    Ctx::Assess& A = c->A;
+    A.n = 0;
+    A.scans = A.skipped = 0;
+    A.last_q = -1;
+    A.last_n = 0;
+    A.timed_scans = A.untimed_scans = 0;
+    A.pool_rows = 0;
+    A.hold_seq = -1;
+    return LIINIT_OK;
+}
+
+int liinit_map_snapshot(liinit_ctx* h, long long* bytes) {
+    if (!h) return LIINIT_ERR_INVALID;
+    Ctx* c = &h->c;
+    if (has_comm(c)) return fail(c, LIINIT_ERR_INVALID, "the map snapshot does not take a communicator (liinit_comm_init)");
+    CU(cudaSetDevice(c->device));
+    return map_snapshot(c, bytes);
+}
+
+int liinit_map_restore(liinit_ctx* h) {
+    if (!h) return LIINIT_ERR_INVALID;
+    Ctx* c = &h->c;
+    CU(cudaSetDevice(c->device));
+    return map_restore(c);
+}
+
+int liinit_replay_reserve(liinit_ctx* h, long long max_points, int max_frames) {
+    if (!h) return LIINIT_ERR_INVALID;
+    Ctx* c = &h->c;
+    if (max_points < 1 || max_points > LIINIT_ASSESS_MAX_POINTS) return fail(c, LIINIT_ERR_INVALID, "max_points must be in [1, LIINIT_ASSESS_MAX_POINTS]");
+    if (max_frames < 1 || max_frames > LIINIT_ASSESS_MAX_SCANS) return fail(c, LIINIT_ERR_INVALID, "max_frames must be in [1, LIINIT_ASSESS_MAX_SCANS]");
+    CU(cudaSetDevice(c->device));
+    CU(cudaStreamSynchronize(c->stream));
+    replay_free(c);
+    Ctx::Replay& R = c->R;
+    if (cudaMalloc(&R.pts, (size_t)max_points * sizeof(float4)) != cudaSuccess || cudaMalloc(&R.inten, (size_t)max_points * sizeof(float)) != cudaSuccess) {
+        cudaGetLastError();
+        replay_free(c);
+        return fail(c, LIINIT_ERR_CUDA, "cudaMalloc of the replay store (" + std::to_string(max_points) + " points) failed");
+    }
+    R.cap = max_points;
+    R.max_frames = max_frames;
+    R.fr.reserve((size_t)(max_frames < 65536 ? max_frames : 65536));
+    return LIINIT_OK;
+}
+
+int liinit_replay_append(liinit_ctx* h, long long handle, double t_beg, float end_ms, int* appended) {
+    if (!h) return LIINIT_ERR_INVALID;
+    Ctx* c = &h->c;
+    if (!appended) return fail(c, LIINIT_ERR_INVALID, "null argument");
+    Ctx::Replay& R = c->R;
+    if (R.cap <= 0) return fail(c, LIINIT_ERR_INVALID, "no replay store (liinit_replay_reserve)");
+    int slot = 0;
+    const FrameSub* s = frame_lookup(c, handle, &slot);
+    if (!s) return fail(c, LIINIT_ERR_INVALID, "unknown sub-frame handle (its message slot has been reused)");
+    CU(cudaSetDevice(c->device));
+    if (R.n + s->n > R.cap || (int)R.fr.size() >= R.max_frames) {
+        R.skipped++;
+        *appended = 0;
+        return LIINIT_OK;
+    }
+    const size_t o = (size_t)slot * c->stage_pts_cap + (s->lo - 1);
+    CU(cudaMemcpyAsync(R.pts + R.n, c->d_fr_slot_pts + o, (size_t)s->n * sizeof(float4), cudaMemcpyDeviceToDevice, c->stream));
+    CU(cudaMemcpyAsync(R.inten + R.n, c->d_fr_slot_inten + o, (size_t)s->n * sizeof(float), cudaMemcpyDeviceToDevice, c->stream));
+    R.fr.push_back(Ctx::ReplayFrame{t_beg, end_ms, s->n, R.n});
+    R.n += s->n;
+    *appended = 1;
+    return LIINIT_OK;
+}
+
+int liinit_replay_info(liinit_ctx* h, int* frames, int* skipped, long long* points) {
+    if (!h) return LIINIT_ERR_INVALID;
+    Ctx* c = &h->c;
+    if (c->R.cap <= 0) return fail(c, LIINIT_ERR_INVALID, "no replay store (liinit_replay_reserve)");
+    if (frames) *frames = (int)c->R.fr.size();
+    if (skipped) *skipped = c->R.skipped;
+    if (points) *points = c->R.n;
+    return LIINIT_OK;
+}
+
+int liinit_replay_frame(liinit_ctx* h, int j, double* t_beg, float* end_ms, int* n) {
+    if (!h) return LIINIT_ERR_INVALID;
+    Ctx* c = &h->c;
+    if (j < 0 || j >= (int)c->R.fr.size()) return fail(c, LIINIT_ERR_INVALID, "no such stored sub-frame");
+    const Ctx::ReplayFrame& f = c->R.fr[j];
+    if (t_beg) *t_beg = f.t_beg;
+    if (end_ms) *end_ms = f.end_ms;
+    if (n) *n = f.n;
+    return LIINIT_OK;
+}
+
+int liinit_replay_stage(liinit_ctx* h, int j) {
+    if (!h) return LIINIT_ERR_INVALID;
+    Ctx* c = &h->c;
+    if (j < 0 || j >= (int)c->R.fr.size()) return fail(c, LIINIT_ERR_INVALID, "no such stored sub-frame");
+    CU(cudaSetDevice(c->device));
+    const Ctx::ReplayFrame& f = c->R.fr[j];
+    // liinit_frame_stage's copy and attribute kernel, from the store instead of the message slot
+    CU(cudaMemcpyAsync(c->d_stage_pts, c->R.pts + f.lo, (size_t)f.n * sizeof(float4), cudaMemcpyDeviceToDevice, c->stream));
+    k_attr_from_inten<<<nblk(f.n, 256), 256, 0, c->stream>>>(c->R.inten + f.lo, f.n, c->d_stage_attr);
+    c->launches++;
+    CU(cudaGetLastError());
+    c->stage_attr = true;
+    c->raw_n = f.n;
+    c->stage_seq++;
+    return LIINIT_OK;
 }
 
 }  // extern "C"

@@ -49,6 +49,10 @@ def load():
     L.liinit_ieskf_update.argtypes = [_f64, _f64, _f64, _f64, _f64, C.c_void_p]
     L.liinit_scan_update.restype = C.c_int
     L.liinit_scan_update.argtypes = [C.c_void_p, _f64, C.c_int, C.c_int, C.POINTER(ScanStats)]
+    L.liinit_ieskf_update_frozen.restype = C.c_int
+    L.liinit_ieskf_update_frozen.argtypes = [_f64, _f64, _f64, _f64, _f64, C.c_void_p]
+    L.liinit_scan_update_frozen.restype = C.c_int
+    L.liinit_scan_update_frozen.argtypes = [C.c_void_p, _f64, C.c_int, C.c_int, C.POINTER(ScanStats)]
     L.liinit_propagate_cv.restype = None
     L.liinit_propagate_cv.argtypes = [_f64, C.c_double, _f64, _f64]
     pimu = C.POINTER(Imu)
@@ -101,11 +105,13 @@ def boxminus(a, b):
     return o
 
 
-def ieskf_update(state, state_prop, HtH, Htr):
+def ieskf_update(state, state_prop, HtH, Htr, frozen=False):
+    """One IESKF update; frozen: the extrinsic held constant (liinit_ieskf_update_frozen)."""
     s = np.ascontiguousarray(state, np.float64).copy()
     sol = np.zeros(24)
     KH = np.zeros((24, 12))
-    rc = load().liinit_ieskf_update(s, np.ascontiguousarray(state_prop, np.float64), np.ascontiguousarray(HtH, np.float64).reshape(144),
+    L = load()
+    rc = (L.liinit_ieskf_update_frozen if frozen else L.liinit_ieskf_update)(s, np.ascontiguousarray(state_prop, np.float64), np.ascontiguousarray(HtH, np.float64).reshape(144),
                                     np.ascontiguousarray(Htr, np.float64), sol, KH.ctypes.data_as(C.c_void_p))
     if rc != 0:
         raise RuntimeError("liinit_ieskf_update failed (singular covariance?)")
@@ -121,11 +127,13 @@ def propagate_cv(state, dt, cov_gyr_scale=0.1, cov_acc_scale=0.1):
     return s
 
 
-def scan_update(gpu: capi.LiInitGpu, state, max_iteration=5, imu_en=False):
-    """Per-scan ICP + IESKF update on the scan already uploaded to `gpu`. Returns (posterior state, stats dict)."""
+def scan_update(gpu: capi.LiInitGpu, state, max_iteration=5, imu_en=False, frozen=False):
+    """Per-scan ICP + IESKF update on the scan already uploaded to `gpu`; frozen: the extrinsic held constant
+    (liinit_scan_update_frozen). Returns (posterior state, stats dict)."""
     s = np.ascontiguousarray(state, np.float64).copy()
     st = ScanStats()
-    rc = load().liinit_scan_update(gpu.h, s, int(max_iteration), int(imu_en), C.byref(st))
+    L = load()
+    rc = (L.liinit_scan_update_frozen if frozen else L.liinit_scan_update)(gpu.h, s, int(max_iteration), int(imu_en), C.byref(st))
     if rc != 0:
         raise capi.LiInitError(rc, (gpu.L.liinit_last_error(gpu.h) or b"").decode())
     return s, {k: getattr(st, k) for k, _ in ScanStats._fields_}

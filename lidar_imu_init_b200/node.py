@@ -218,6 +218,7 @@ class Node:
         self.on_update = None                       # callback(node) after every update's output rows, for tests and tools
         self.recorder = None                        # a Recorder: the published topics of every update go to its bag
         self.assess = None                          # an assess.Assessment: every LIO update but the switch scan stores its cloud
+        self.replay = None                          # an assess.Replay: captures the hand-over, records the LIO phase's input and updates
         self.debug_logs = None                      # open_debug_logs(): {file name: open file} of LI_Init's logs
         self.closed = False
 
@@ -258,6 +259,8 @@ class Node:
             self.log.warn("IMU loop back, clear IMU buffer.")
             o.calib.clear_imu_all()                 # Init_LI->IMU_buffer_clear() (:420)
         ib.push(stamp, gyr, acc)
+        if self.replay is not None:
+            self.replay.record_imu(stamp, gyr, acc)
         if not o.imu_en and not o.data_accum_finished:
             o.push_imu(gyr, acc, ib.last_stamp, self.cfg.mean_acc_norm)   # push_ALL_IMU_CalibState (:428-430)
 
@@ -313,6 +316,8 @@ class Node:
                 self.assess.append_timed(R, p, RLI, TLI, *timing)   # the scan's raw cloud, pose table and propagated state
             else:
                 self.assess.append(R, p, RLI, TLI)
+        if self.replay is not None:
+            self.replay.record_update(s)
         if self.on_update is not None:               # the posterior of the update, before the hand-over of a trigger scan
             self.on_update(self)
         # the refinement clock (:1169-1187)
@@ -336,6 +341,8 @@ class Node:
             if self.debug_logs is not None:
                 self._write_debug_logs()
             self.online_calib_starts_time = t
+            if self.replay is not None:
+                self.replay.capture(o, res)         # the LiDAR-only state and the map as LI-Init found them
             o.hand_over(res)
             self.init_scan = o.frame_num
             self.init_state = o.state.copy()

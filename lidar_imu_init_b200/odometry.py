@@ -90,6 +90,13 @@ class SubFrame:
         self.n = int(entry["n"])
 
 
+class ReplayFrame(SubFrame):
+    """A sub-frame of the replay store (liinit_replay_*): stored sub-frame j, staged by liinit_replay_stage."""
+
+    def __init__(self, j: int, end_ms, n: int):
+        self.j, self.end_ms, self.n = int(j), np.float32(end_ms), int(n)
+
+
 class LidarOdometry:
     def __init__(self, gpu: capi.LiInitGpu, filter_size_map: float, max_iteration: int = 4, gyr_cov: float = 0.1, acc_cov: float = 0.1,
                  orig_odom_freq: int = 10, cut_frame_num: int = 1, data_accum_length: float = 300.0, calib: LiCalib | None = None,
@@ -140,6 +147,10 @@ class LidarOdometry:
         # timing keeps (pose table, propagated state) of the last process_raw that undistorted from a table (None for any other)
         self.assess_hold = False
         self.timing = None
+        # a replay of the LIO phase (assess.Replay): process_next hands it every sub-frame it processes; frozen: the update holds the
+        # extrinsic constant (liinit_scan_update_frozen)
+        self.replay = None
+        self.frozen = False
 
     def push_imu(self, omg, acc, t, mean_acc_norm=9.81):
         """imu_cbk in LO mode (:428-430)."""
@@ -291,6 +302,8 @@ class LidarOdometry:
             return None
         self.lidar_buffer.popleft()
         group = self.imu_buffer.pop(t_end)
+        if self.replay is not None:
+            self.replay.record_frame(e)
         return self.process_raw(SubFrame(e), e["t_beg"], group)
 
     def _publish(self, R, p, RLI, TLI):
@@ -364,8 +377,11 @@ class LidarOdometry:
         return self.imu_proc.propagate(state, group, t_beg, end_ms)
 
     def _stage(self, raw):
-        """Stage the raw cloud of the scan: an uploaded PointType array, or a sub-frame the device already holds."""
-        if isinstance(raw, SubFrame):
+        """Stage the raw cloud of the scan: an uploaded PointType array, or a sub-frame the device already holds (in a message slot or
+        in the replay store)."""
+        if isinstance(raw, ReplayFrame):
+            self.g.replay_stage(raw.j)
+        elif isinstance(raw, SubFrame):
             self.g.frame_stage(raw.handle)
         else:
             self.g.raw_upload(raw, 9)
@@ -389,7 +405,7 @@ class LidarOdometry:
         return self.g.scan_body()
 
     def _scan_update_resident(self, state):
-        return host.scan_update(self.g, state, self.max_iteration, self.imu_en)
+        return host.scan_update(self.g, state, self.max_iteration, self.imu_en, frozen=self.frozen)
 
     def hand_over(self, res):
         """laserMapping.cpp:1198-1222 after LI_Initialization: the pose is re-expressed in the IMU frame with the calibrated extrinsic,

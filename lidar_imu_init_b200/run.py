@@ -4,7 +4,7 @@
                                       [--max-map-points N] [--record PATH [--record-format ros1|ros2]
                                       [--record-compression none|bz2] [--record-topics a,b,...]] [--debug-logs]
                                       [--assess] [--assess-cloud PATH [--assess-cloud-leaf L]] [--assess-radius R]
-                                      [--assess-max-points N] [--assess-time]
+                                      [--assess-max-points N] [--assess-time] [--assess-replay [--assess-replay-max-points N]]
 
 --bag is a ROS1 bag (v2.0), a rosbag2 directory (sqlite3 storage) or one of its .db3 files, told apart by the file's first bytes. The
 LiDAR topic carries livox_ros_driver/CustomMsg or livox_ros_driver2/CustomMsg (lidar_type 1) or sensor_msgs/PointCloud2 in a ROS1
@@ -25,6 +25,10 @@ map entropy and plane variance of the as-run, final and perturbed extrinsics, wr
 point, averaged over cubic leaves of --assess-cloud-leaf metres (0: every point), as a binary PCD.
 --assess-time also keeps each LIO scan's raw cloud and IMU pose table, re-undistorts the scans for every candidate, and scores the
 time lag too: the 14 candidates and a lag profile around the run's lag, written to DIR/result/assessment_time.txt.
+--assess-replay keeps the map at the hand-over and the LIO phase's sub-frames and IMU samples, and runs the LIO phase again for every
+candidate with the candidate extrinsic held constant: the run itself, LI-Init's result, the final extrinsic, its 12 perturbations and
+the final extrinsic at lag shifts of -+5 ms, each scored by the sharpness of the map its replay builds, written to
+DIR/result/assessment_replay.txt (stores the LIO scans like --assess).
 """
 from __future__ import annotations
 
@@ -72,6 +76,12 @@ def parse_args(argv=None):
                     help=f"LIO points the assessment stores on the device (default {assessmod.MAX_POINTS}); later scans are skipped")
     ap.add_argument("--assess-time", action="store_true", help="score the time lag too, re-undistorting the stored LIO scans for every "
                     "candidate: DIR/result/assessment_time.txt (stores the LIO scans like --assess)")
+    ap.add_argument("--assess-replay", action="store_true", help="run the LIO phase again for every candidate calibration, extrinsic "
+                    "held constant, and score the map each replay builds: DIR/result/assessment_replay.txt (stores the LIO scans like "
+                    "--assess)")
+    ap.add_argument("--assess-replay-max-points", type=int, default=assessmod.REPLAY_MAX_POINTS, metavar="N",
+                    help=f"raw LIO-phase points the replay keeps on the device (default {assessmod.REPLAY_MAX_POINTS}); a run that "
+                    "outgrows it is not replayed")
     return ap.parse_args(argv)
 
 
@@ -99,7 +109,7 @@ def make_node(args, cfg, log):
 
 def main(argv=None, on_node=None) -> int:
     """The command line; on_node(node), when given, is called with the Node before the bag is played (for tools and tests)."""
-    from . import capi, calib
+    from . import calib, capi, host
     from .node import Log, Recorder
     args = parse_args(argv)
     log = Log(quiet=args.quiet)
@@ -107,13 +117,15 @@ def main(argv=None, on_node=None) -> int:
     try:
         cfg = cfgmod.load(args.config, args.param)
         topics = record_topics(args)
-        assessing = args.assess or args.assess_cloud is not None or args.assess_time
+        assessing = args.assess or args.assess_cloud is not None or args.assess_time or args.assess_replay
         if assessing and not (args.assess_radius > 0 and args.assess_radius < float("inf")):
             raise cfgmod.ConfigError(f"--assess-radius {args.assess_radius!r}: must be a positive number of metres")
         if args.assess_cloud is not None and not (args.assess_cloud_leaf >= 0 and args.assess_cloud_leaf < float("inf")):
             raise cfgmod.ConfigError(f"--assess-cloud-leaf {args.assess_cloud_leaf!r}: must be zero or a positive number of metres")
         if assessing and args.assess_max_points < 1:
             raise cfgmod.ConfigError(f"--assess-max-points {args.assess_max_points}: must be positive")
+        if args.assess_replay and args.assess_replay_max_points < 1:
+            raise cfgmod.ConfigError(f"--assess-replay-max-points {args.assess_replay_max_points}: must be positive")
         with rosbag2.open_bag(args.bag) as bag:
             bag.check_topics(cfgmod.wanted_topics(cfg, bag.format))
             if args.record:
@@ -128,6 +140,8 @@ def main(argv=None, on_node=None) -> int:
             if assessing:
                 node.assess = assessmod.Assessment(node.odom.g, args.assess_max_points, args.assess_radius, timed=args.assess_time)
                 node.odom.assess_hold = args.assess_time
+            if args.assess_replay:
+                node.replay = node.odom.replay = assessmod.Replay(node.odom.g, node.assess, args.assess_replay_max_points)
             if on_node is not None:
                 on_node(node)
             t0 = time.perf_counter()
@@ -151,10 +165,17 @@ def main(argv=None, on_node=None) -> int:
             else:
                 log.info(f"assessment cloud written to {args.assess_cloud}: {got[0]} records, full-resolution MME {got[1]['mme']:.6f} over "
                          f"{got[1]['valid']} of {got[1]['points']} points, in {time.perf_counter() - t0:.1f} s")
+        if args.assess_replay:
+            # (last: every replay refills the assessment store)
+            t0 = time.perf_counter()
+            path = os.path.join(args.out, "result", "assessment_replay.txt")
+            _, _, R_final, T_final = host.state_pose(node.odom.state)
+            node.replay.write(path, R_final, T_final)
+            log.info(f"replay assessment written to {path} in {time.perf_counter() - t0:.1f} s")
         node.odom.g.close()
         log.info(f"{node.updates} updates in {wall:.1f} s; {node.odom.dropped_subframes} sub-frames dropped")
         return 0
-    except (cfgmod.ConfigError, rosbag.BagError, rosmsg.MsgError, capi.LiInitError, calib.CalibError, OSError) as e:
+    except (cfgmod.ConfigError, rosbag.BagError, rosmsg.MsgError, capi.LiInitError, calib.CalibError, assessmod.ReplayError, OSError) as e:
         _abort(node, writer)
         sys.stderr.write(f"error: {e}\n")
         return 1
