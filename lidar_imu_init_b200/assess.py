@@ -393,6 +393,53 @@ class Replay:
         with open(path, "w") as f:
             f.write(NOTHING if self.base is None or not self.frames else self.report(R_final, T_final))
 
+    @property
+    def lag(self) -> float:
+        """The node's total lag at the hand-over, time_lag_IMU_wtr_lidar + timediff_imu_wrt_lidar [s]; a replay's lag shift adds to it."""
+        return float(self.base.imu_buffer.timediff) + float(self.res["time_lag_1"]) + float(self.res["time_lag_2"])
+
+    def refine(self, R_final, T_final, max_replays=None) -> dict:
+        """refine.search with frozen replays as the scorer, from the run's final extrinsic and LI-Init's at shift 0. Returns search's
+        dict with, on every trace row, the replay's "result" (the as-run evaluation) and "seconds"; and "wall_s", "lag0" (the lag at the
+        hand-over [s]), "time_lag" (the refined total lag [s]), "state" (the best replay's last posterior state, whose extrinsic is the
+        refined one) and "calib" (node.state_calib_values of that state and lag, the arguments of node.calib_result_text)."""
+        import time
+
+        from . import refine as rf
+        from .node import state_calib_values
+        kept = {}
+
+        def score(R, T, shift_s):
+            r = self.run(R, T, shift_s, frozen=True)
+            kept[rf.key(R, T, shift_s)] = (r["result"], r["seconds"], r["states"][-1][1] if r["states"] else None)
+            return r["result"]["mme"]
+        t0 = time.perf_counter()
+        out = rf.search(score, R_final, T_final, 0.0, rf.MAX_REPLAYS if max_replays is None else max_replays,
+                        R_init=self.res["R_LI"], T_init=self.res["T_LI"])
+        out["wall_s"] = time.perf_counter() - t0
+        for row in out["trace"]:
+            row["result"], row["seconds"], _ = kept[rf.key(row["R"], row["T"], row["shift_ms"] / 1000.0)]
+        state = kept[rf.key(out["R"], out["T"], out["shift_s"])][2]
+        if state is None:
+            raise ReplayError("the best replay made no LIO update: nothing to take the biases and gravity from")
+        out["lag0"] = self.lag
+        out["time_lag"] = self.lag + out["shift_s"]
+        out["state"] = state
+        out["calib"] = state_calib_values(state, out["time_lag"])
+        return out
+
+    def write_refinement(self, path: str, R_final=None, T_final=None, max_replays=None):
+        """result/refinement.txt (refine_report_text); R_final / T_final: the run's final extrinsic. Returns refine's dict, or None,
+        writing NOTHING, when the run did not hand over."""
+        if self.base is None or not self.frames:
+            with open(path, "w") as f:
+                f.write(NOTHING)
+            return None
+        ref = self.refine(R_final, T_final, max_replays)
+        with open(path, "w") as f:
+            f.write(refine_report_text(self.info(), ref, self.assessment.radius, self.assessment.min_neighbors))
+        return ref
+
 
 def host_pose(state):
     from . import host
@@ -457,3 +504,60 @@ def parse_replay_report(text: str) -> dict:
     f = ls[-1].split()
     assert f[0] == "lag" and f[2] == "best_shift_ms" and f[4] == "d_minus" and f[6] == "d_plus", ls[-1]
     return {"header": header, "rows": rows, "axes": axes, "lag": (f[1], float(f[3]), float(f[5]), float(f[7]))}
+
+
+REFINED = "Refined result:"
+_REFINE_INT = ("subframes", "skipped", "replays", "at_edge", "n_min", "valid", "sparse", "degenerate")
+
+
+def refine_report_text(info: dict, ref: dict, radius: float, min_neighbors: int) -> str:
+    """result/refinement.txt of Replay.refine's dict: a header line of key value pairs (the replay store's sub-frames and skipped ones,
+    the start candidate, the replays, the wall time, converged or budget, whether stage 1's lag minimum lay at the cap, the lag at the
+    hand-over, the refined lag shift and total lag, the score's radius and n_min), a column line, one fixed-column row per replay in
+    evaluation order (its stage, the candidate, its lag shift, the as-run score of the map it built and its time), one line per axis (its
+    verdict, the final step [deg or m] and the MME differences of its + and - neighbours at that step to the refined candidate), then
+    `Refined result:` and node.calib_result_text."""
+    from .node import calib_result_text, rot_to_euler
+    from .refine import axis_verdict
+    lines = [f"subframes {info['frames']} skipped {info['skipped']} start {ref['start']} replays {len(ref['trace'])} "
+             f"wall_s {ref['wall_s']:.6f} status {ref['status']} at_edge {int(ref['at_edge'])} lag0_ms {ref['lag0'] * 1000.0:.6f} "
+             f"shift_ms {ref['shift_ms']:.6f} lag_ms {ref['time_lag'] * 1000.0:.6f} radius {radius:.6f} n_min {min_neighbors}",
+             "%-7s %11s %11s %11s %10s %10s %10s %11s %10s %10s %10s %15s %15s %9s" % (
+                 "stage", "roll_deg", "pitch_deg", "yaw_deg", "t_x", "t_y", "t_z", "shift_ms", "valid", "sparse", "degenerate", "mme", "mpv",
+                 "seconds")]
+    for r in ref["trace"]:
+        e, T, res = np.degrees(rot_to_euler(r["R"])), r["T"], r["result"]
+        lines.append("%-7s %11.6f %11.6f %11.6f %10.6f %10.6f %10.6f %11.6f %10d %10d %10d %15.9f %15.9e %9.3f" % (
+            r["stage"], e[0], e[1], e[2], T[0], T[1], T[2], r["shift_ms"], res["valid"], res["sparse"], res["degenerate"], res["mme"],
+            res["mpv"], r["seconds"]))
+    for axis, (step, dp, dm) in ref["axes"].items():
+        lines.append("%-7s %-11s %12.6f %15.9f %15.9f" % (axis, axis_verdict(dp, dm), step, dp, dm))
+    return "\n".join(lines) + "\n" + REFINED + "\n" + calib_result_text(**ref["calib"])
+
+
+def parse_refine_report(text: str) -> dict:
+    """The inverse of refine_report_text: {"header": {...}, "rows": [{"stage", ...}] in evaluation order, "axes": {axis: (verdict, step,
+    d_plus, d_minus)}, "result": the calib_result_text block}, or {"nothing": True}."""
+    if text == NOTHING:
+        return {"nothing": True}
+    head, result = text.split("\n" + REFINED + "\n", 1)
+    ls = head.splitlines()
+
+    def val(x):
+        for t in (int, float):
+            try:
+                return t(x)
+            except ValueError:
+                pass
+        return x
+    h = ls[0].split()
+    header = {h[i]: val(h[i + 1]) for i in range(0, len(h), 2)}
+    cols = ls[1].split()
+    n = header["replays"]
+    rows = [{c: (x if c == "stage" else int(x) if c in _REFINE_INT else float(x)) for c, x in zip(cols, line.split())}
+            for line in ls[2:2 + n]]
+    axes = {}
+    for line in ls[2 + n:]:
+        f = line.split()
+        axes[f[0]] = (f[1], float(f[2]), float(f[3]), float(f[4]))
+    return {"header": header, "rows": rows, "axes": axes, "result": result}

@@ -4,7 +4,8 @@
                                       [--max-map-points N] [--record PATH [--record-format ros1|ros2]
                                       [--record-compression none|bz2] [--record-topics a,b,...]] [--debug-logs]
                                       [--assess] [--assess-cloud PATH [--assess-cloud-leaf L]] [--assess-radius R]
-                                      [--assess-max-points N] [--assess-time] [--assess-replay [--assess-replay-max-points N]]
+                                      [--assess-max-points N] [--assess-time] [--assess-replay] [--assess-replay-max-points N]
+                                      [--refine [--refine-max-replays N]]
 
 --bag is a ROS1 bag (v2.0), a rosbag2 directory (sqlite3 storage) or one of its .db3 files, told apart by the file's first bytes. The
 LiDAR topic carries livox_ros_driver/CustomMsg or livox_ros_driver2/CustomMsg (lidar_type 1) or sensor_msgs/PointCloud2 in a ROS1
@@ -29,6 +30,10 @@ time lag too: the 14 candidates and a lag profile around the run's lag, written 
 candidate with the candidate extrinsic held constant: the run itself, LI-Init's result, the final extrinsic, its 12 perturbations and
 the final extrinsic at lag shifts of -+5 ms, each scored by the sharpness of the map its replay builds, written to
 DIR/result/assessment_replay.txt (stores the LIO scans like --assess).
+--refine records the LIO phase as --assess-replay does and searches, by replay, for the lag shift and then the extrinsic whose map is
+sharpest, starting from the better of LI-Init's result and the final extrinsic, within --refine-max-replays replays (default 120). It
+writes every replay, the end condition of each axis and the refined calibration, in the format of Initialization_result.txt, to
+DIR/result/refinement.txt, and leaves Initialization_result.txt as it is.
 """
 from __future__ import annotations
 
@@ -40,6 +45,7 @@ import time
 from . import assess as assessmod
 from . import bagwrite
 from . import config as cfgmod
+from . import refine as refinemod
 from . import rosbag, rosbag2, rosmsg
 
 
@@ -82,7 +88,23 @@ def parse_args(argv=None):
     ap.add_argument("--assess-replay-max-points", type=int, default=assessmod.REPLAY_MAX_POINTS, metavar="N",
                     help=f"raw LIO-phase points the replay keeps on the device (default {assessmod.REPLAY_MAX_POINTS}); a run that "
                     "outgrows it is not replayed")
+    ap.add_argument("--refine", action="store_true", help="search, by LIO replay, for the lag and extrinsic whose map is sharpest and "
+                    "write the refined calibration: DIR/result/refinement.txt (records the replay like --assess-replay)")
+    ap.add_argument("--refine-max-replays", metavar="N", help=f"replays the refinement may spend (default {refinemod.MAX_REPLAYS})")
     return ap.parse_args(argv)
+
+
+def refine_max_replays(args) -> int:
+    """--refine-max-replays as a positive integer (refine.MAX_REPLAYS when it is not given)."""
+    if args.refine_max_replays is None:
+        return refinemod.MAX_REPLAYS
+    try:
+        n = int(args.refine_max_replays)
+    except ValueError:
+        n = 0
+    if n < 1:
+        raise cfgmod.ConfigError(f"--refine-max-replays {args.refine_max_replays!r}: must be a positive integer")
+    return n
 
 
 def record_topics(args) -> tuple:
@@ -117,15 +139,17 @@ def main(argv=None, on_node=None) -> int:
     try:
         cfg = cfgmod.load(args.config, args.param)
         topics = record_topics(args)
-        assessing = args.assess or args.assess_cloud is not None or args.assess_time or args.assess_replay
+        replaying = args.assess_replay or args.refine
+        assessing = args.assess or args.assess_cloud is not None or args.assess_time or replaying
         if assessing and not (args.assess_radius > 0 and args.assess_radius < float("inf")):
             raise cfgmod.ConfigError(f"--assess-radius {args.assess_radius!r}: must be a positive number of metres")
         if args.assess_cloud is not None and not (args.assess_cloud_leaf >= 0 and args.assess_cloud_leaf < float("inf")):
             raise cfgmod.ConfigError(f"--assess-cloud-leaf {args.assess_cloud_leaf!r}: must be zero or a positive number of metres")
         if assessing and args.assess_max_points < 1:
             raise cfgmod.ConfigError(f"--assess-max-points {args.assess_max_points}: must be positive")
-        if args.assess_replay and args.assess_replay_max_points < 1:
+        if replaying and args.assess_replay_max_points < 1:
             raise cfgmod.ConfigError(f"--assess-replay-max-points {args.assess_replay_max_points}: must be positive")
+        max_replays = refine_max_replays(args) if args.refine else None
         with rosbag2.open_bag(args.bag) as bag:
             bag.check_topics(cfgmod.wanted_topics(cfg, bag.format))
             if args.record:
@@ -140,7 +164,7 @@ def main(argv=None, on_node=None) -> int:
             if assessing:
                 node.assess = assessmod.Assessment(node.odom.g, args.assess_max_points, args.assess_radius, timed=args.assess_time)
                 node.odom.assess_hold = args.assess_time
-            if args.assess_replay:
+            if replaying:
                 node.replay = node.odom.replay = assessmod.Replay(node.odom.g, node.assess, args.assess_replay_max_points)
             if on_node is not None:
                 on_node(node)
@@ -172,6 +196,15 @@ def main(argv=None, on_node=None) -> int:
             _, _, R_final, T_final = host.state_pose(node.odom.state)
             node.replay.write(path, R_final, T_final)
             log.info(f"replay assessment written to {path} in {time.perf_counter() - t0:.1f} s")
+        if args.refine:
+            # (after --assess-replay: every replay refills the assessment store)
+            path = os.path.join(args.out, "result", "refinement.txt")
+            _, _, R_final, T_final = host.state_pose(node.odom.state)
+            ref = node.replay.write_refinement(path, R_final, T_final, max_replays)
+            if ref is None:
+                log.warn(f"{path}: {assessmod.NOTHING.strip()}")
+            else:
+                log.info(refine_summary(path, ref))
         node.odom.g.close()
         log.info(f"{node.updates} updates in {wall:.1f} s; {node.odom.dropped_subframes} sub-frames dropped")
         return 0
@@ -183,6 +216,16 @@ def main(argv=None, on_node=None) -> int:
         # an interrupted run (Ctrl-C) still closes its files and its recording, so the bag it leaves is complete
         _abort(node, writer)
         raise
+
+
+def refine_summary(path: str, ref: dict) -> str:
+    """The refinement's summary line: the lag, extrinsic change and MME from the start candidate to the refined one."""
+    import numpy as np
+    s = ref["trace"][[r["stage"] for r in ref["trace"]].index(ref["start"])]
+    c = np.clip((np.trace(ref["R"] @ s["R"].T) - 1.0) / 2.0, -1.0, 1.0)
+    return (f"refinement written to {path}: {len(ref['trace'])} replays in {ref['wall_s']:.1f} s ({ref['status']}); lag "
+            f"{ref['lag0'] * 1000.0:.3f} -> {ref['time_lag'] * 1000.0:.3f} ms; from {ref['start']}: rotation {np.degrees(np.arccos(c)):.4f} deg, "
+            f"translation {np.linalg.norm(ref['T'] - s['T']) * 1000.0:.2f} mm; MME {s['mme']:.6f} -> {ref['mme']:.6f}")
 
 
 def _abort(node, writer):
