@@ -8,9 +8,15 @@
  *
  * Conventions: extern "C"; opaque context; int return codes (0 = LIINIT_OK, <0 =
  * error, message via liinit_last_error); no exceptions cross the ABI; the caller
- * owns every host buffer, the library owns all device memory; single caller thread
- * (the node's main thread, laserMapping.cpp:891-1238), internally asynchronous on
- * one CUDA stream. Matrices are row-major doubles. Point arrays are float with a
+ * owns every host buffer, the library owns all device memory; one thread at a time
+ * per context (the node drives its one context from its main thread,
+ * laserMapping.cpp:891-1238); distinct contexts may be driven from distinct threads
+ * at once. Each context is internally asynchronous on its own non-blocking CUDA
+ * stream. (What makes that safe: the library keeps no process-wide state on any
+ * path but liinit_create's error text, which is thread_local, and the lazy dlopen of
+ * NCCL behind liinit_comm_*; the host library, liinit_host.h, keeps none at all.
+ * A call that names two contexts -- liinit_replay_share -- counts as a call on
+ * both.) Matrices are row-major doubles. Point arrays are float with a
  * caller-given stride in floats: 3 (packed xyz), 4 (float4) or 12 (the 48-byte
  * pcl::PointXYZINormal of include/common_lib.h:37 -- x,y,z are its first floats).
  *
@@ -446,6 +452,20 @@ int liinit_replay_info(liinit_ctx* h, int* frames, int* skipped, long long* poin
 int liinit_replay_frame(liinit_ctx* h, int j, double* t_beg, float* end_ms, int* n);
 /* Stages stored sub-frame j as the raw cloud, exactly as liinit_frame_stage staged the original. */
 int liinit_replay_stage(liinit_ctx* h, int j);
+/* Concurrent replays: one context per replay, all reading one store. After liinit_replay_share(worker, lead), the worker's
+ * liinit_map_restore copies from the lead's snapshot and its liinit_replay_info / _frame / _stage read the lead's store. The pointers
+ * are not owned: the worker allocates no copy of either. The call synchronises the lead's stream once, so the store and the snapshot
+ * are complete before any worker's stream reads them; each context then runs on its own stream, and a worker and its lead (or two
+ * workers) may be driven from distinct threads at once. The worker keeps its own map, staged cloud, resident scan and assessment store.
+ * LIINIT_ERR_INVALID, with a message, when: worker == lead; they are on different devices; their configurations differ (hash slots,
+ * brick cells, cell directory on or off, capacities, filter_size_map); either has a communicator; the worker already shares or is
+ * itself a lead; the lead shares another's; the lead has no snapshot or no replay store.
+ * While shared: on the lead, liinit_map_snapshot, liinit_replay_reserve, liinit_replay_append and liinit_destroy are refused; on the
+ * worker, liinit_map_snapshot, liinit_replay_reserve and liinit_replay_append are refused (LIINIT_ERR_INVALID).
+ * liinit_replay_unshare (LIINIT_ERR_INVALID when the context does not share) and liinit_destroy of the worker end the sharing; both
+ * first synchronise the worker's stream. */
+int liinit_replay_share(liinit_ctx* worker, liinit_ctx* lead);
+int liinit_replay_unshare(liinit_ctx* worker);
 
 #ifdef __cplusplus
 }

@@ -281,15 +281,23 @@ class Replay:
         self.base = None          # the LidarOdometry before the hand-over (a copy)
         self.res = None           # LI-Init's result
         self.snapshot_bytes = 0
+        self.staged_points = 0    # points of the raw cloud staged at the snapshot (the first updates may store it again)
         self.events = []          # after the hand-over, in arrival order: stored sub-frame index (int) or IMU sample (stamp, gyr, acc)
         self.frames = 0
         self.run_states = []      # (stored sub-frame index, posterior state) of the run's updates after the hand-over
+        # concurrent replays (run_many): worker contexts that share this context's replay store and map snapshot, created once
+        self.workers = []
+        self.jobs = 1             # replays at once of write() and write_refinement()
+        self.threads = None       # threads of a batch; None: one per context (a CPU build of the kernels needs 1)
+        self.host_lib = None      # the host library that runs the native loop (None: the package's)
+        self._recorded = None     # (IMU samples [k, 7], int32 event codes) of self.events for the native loop
 
     # ---- recording ----
     def capture(self, odom, res):
         if self.base is not None:
             raise ReplayError("the hand-over has been captured already")
         self.snapshot_bytes = self.g.map_snapshot()
+        self.staged_points = int(getattr(self.g, "raw_n", 0))
         self.base = _clone_odometry(odom)
         self.res = dict(res)
 
@@ -325,21 +333,7 @@ class Replay:
             raise ReplayError(f"the replay store is truncated ({info['skipped']} sub-frames skipped): raise its max_points")
         t0 = time.perf_counter()
         frames = [self.g.replay_frame(j) for j in range(info["frames"])]
-        res = dict(self.res)
-        if R_LI is not None:
-            res["R_LI"], res["T_LI"] = np.asarray(R_LI, float).reshape(3, 3), np.asarray(T_LI, float).reshape(3)
-        res["time_lag_2"] = float(res["time_lag_2"]) + float(lag_shift)
-        o = _clone_odometry(self.base)
-        self.g.map_restore()
-        o.hand_over(res)
-        if frozen:
-            o.frozen = True
-            cov = o.state[36:].reshape(24, 24)
-            cov[6:12, :] = 0.0
-            cov[:, 6:12] = 0.0
-            o.imu_proc.set_cov("R_LI_cov", 0.0)
-            o.imu_proc.set_cov("T_LI_cov", 0.0)
-        self.g.assess_clear()
+        o = self._hand_over(self.g, R_LI, T_LI, lag_shift, frozen)
         states = []
         pending = deque()
         for ev in self.events:
@@ -367,55 +361,175 @@ class Replay:
         return dict(result=result, states=states, R_LI=rli, T_LI=tli, rms_m=trajectory_rms(self.run_states, states),
                     seconds=time.perf_counter() - t0)
 
-    def sweep(self, R_final, T_final, dtheta_deg=DTHETA_DEG, dt=DT_M, lag_ms=REPLAY_LAG_MS) -> list:
+    def _hand_over(self, g, R_LI, T_LI, lag_shift, frozen):
+        """The start of a replay on context g: the map restored, a copy of the captured odometry handed over with the candidate extrinsic
+        (None: LI-Init's) and lag shift [s], for a frozen replay the extrinsic's covariance and propagation noise zeroed, the assessment
+        store emptied. Returns the odometry."""
+        res = dict(self.res)
+        if R_LI is not None:
+            res["R_LI"], res["T_LI"] = np.asarray(R_LI, float).reshape(3, 3), np.asarray(T_LI, float).reshape(3)
+        res["time_lag_2"] = float(res["time_lag_2"]) + float(lag_shift)
+        o = _clone_odometry(self.base)
+        o.g = g
+        g.map_restore()
+        o.hand_over(res)
+        if frozen:
+            o.frozen = True
+            cov = o.state[36:].reshape(24, 24)
+            cov[6:12, :] = 0.0
+            cov[:, 6:12] = 0.0
+            o.imu_proc.set_cov("R_LI_cov", 0.0)
+            o.imu_proc.set_cov("T_LI_cov", 0.0)
+        g.assess_clear()
+        return o
+
+    def run_native(self, R_LI=None, T_LI=None, lag_shift: float = 0.0, frozen: bool = True, g=None) -> dict:
+        """run() with the loop after the hand-over in native code (host.replay_run), on context g: this one (None) or a worker of
+        run_many. Returns run()'s dict, bit for bit."""
+        import time
+
+        from . import host
+        if self.base is None:
+            raise ReplayError("nothing to replay: the run did not reach the hand-over")
+        g = self.g if g is None else g
+        info = self.info()
+        if info["skipped"]:
+            raise ReplayError(f"the replay store is truncated ({info['skipped']} sub-frames skipped): raise its max_points")
+        if not self.base.map_ready:
+            raise ReplayError("nothing to replay: the map was not built at the hand-over")
+        t0 = time.perf_counter()
+        if self._recorded is None or self._recorded[2] != len(self.events):
+            imu = [e for e in self.events if not isinstance(e, int)]
+            samples = np.array([np.concatenate([[t], gyr, acc]) for t, gyr, acc in imu], np.float64).reshape(-1, 7)
+            codes = np.array([e if isinstance(e, int) else host.REPLAY_IMU for e in self.events], np.int32)
+            self._recorded = (samples, codes, len(self.events))
+        o = self._hand_over(g, R_LI, T_LI, lag_shift, frozen)
+        states = host.replay_run(g, o, self._recorded[0], self._recorded[1], lib=self.host_lib)
+        if g is not self.g and g.assess_info()["skipped"]:
+            raise ReplayError("a replay worker's assessment store overflowed: replay with one job")
+        a = self.assessment
+        result = g.assess_evaluate(radius=a.radius, min_neighbors=a.min_neighbors, as_run=True)
+        _, _, rli, tli = host_pose(states[-1][1] if states else o.state)
+        return dict(result=result, states=states, R_LI=rli, T_LI=tli, rms_m=trajectory_rms(self.run_states, states),
+                    seconds=time.perf_counter() - t0)
+
+    def pool(self, jobs: int) -> list:
+        """The contexts of a batch of `jobs` concurrent replays: this one and jobs - 1 workers. A worker is a context of this one's
+        configuration that shares its replay store and map snapshot (liinit_replay_share), with an assessment store sized to the replay
+        store's points and frames; workers are created on first need and kept until close()."""
+        if isinstance(jobs, bool) or int(jobs) != jobs or jobs < 1:
+            raise ValueError(f"replay jobs {jobs!r}: must be a positive integer")
+        if self.base is None:
+            raise ReplayError("nothing to replay: the run did not reach the hand-over")
+        info = self.info()
+        while len(self.workers) < jobs - 1:
+            w = self.g.twin()
+            try:
+                w.replay_share(self.g)
+                w.assess_reserve(info["points"] + self.staged_points, info["frames"] + 1)
+            except BaseException:
+                w.close()
+                raise
+            self.workers.append(w)
+        return [self.g] + self.workers[:jobs - 1]
+
+    def run_many(self, cands, jobs: int = 1, threads=None, native=None) -> list:
+        """Every candidate (R_LI, T_LI, lag_shift [s], frozen) replayed on the contexts of pool(jobs), one thread per context taking
+        the candidates in list order. Returns run()'s dicts in list order; "seconds" is each replay's own wall time. native (default:
+        jobs > 1): the native loop (run_native), else run() on this context. threads (default self.threads, else one per context): 1
+        drives the contexts in turn from the calling thread."""
+        import threading
+        cands = list(cands)
+        ctxs = self.pool(jobs)
+        if not (jobs > 1 if native is None else native):
+            return [self.run(*c) for c in cands]
+        threads = self.threads if threads is None else threads
+        threads = len(ctxs) if threads is None else min(int(threads), len(ctxs))
+        out = [None] * len(cands)
+        if threads <= 1 or len(cands) <= 1:
+            for i, c in enumerate(cands):
+                out[i] = self.run_native(*c, g=ctxs[i % len(ctxs)])
+            return out
+        lock, nxt, errors = threading.Lock(), iter(range(len(cands))), []
+
+        def work(g):
+            while True:
+                with lock:
+                    i = None if errors else next(nxt, None)
+                if i is None:
+                    return
+                try:
+                    out[i] = self.run_native(*cands[i], g=g)
+                except BaseException as e:
+                    with lock:
+                        errors.append((i, e))
+                    return
+        ts = [threading.Thread(target=work, args=(g,)) for g in ctxs[:threads]]
+        for t in ts:
+            t.start()
+        for t in ts:
+            t.join()
+        if errors:
+            raise min(errors, key=lambda x: x[0])[1]
+        return out
+
+    def close(self):
+        """Destroy the workers (the context they share can then be destroyed)."""
+        while self.workers:
+            self.workers.pop().close()
+
+    def sweep(self, R_final, T_final, dtheta_deg=DTHETA_DEG, dt=DT_M, lag_ms=REPLAY_LAG_MS, jobs: int = 1) -> list:
         """[(name, R_LI, T_LI, shift_ms, replay)] of the 17 replays: the run itself (not frozen), LI-Init's result, the final extrinsic,
-        its 12 perturbations, and the final extrinsic at lag shifts of -+lag_ms; all frozen but the first."""
+        its 12 perturbations, and the final extrinsic at lag shifts of -+lag_ms; all frozen but the first. jobs: replays at once
+        (run_many)."""
         R_init = np.asarray(self.res["R_LI"], float).reshape(3, 3)
         T_init = np.asarray(self.res["T_LI"], float).reshape(3)
         plan = [("run", R_init, T_init, 0.0, False), ("li-init", R_init, T_init, 0.0, True)]
         plan += [(name, R, T, 0.0, True) for name, R, T in candidates(R_final, T_final, dtheta_deg, dt)[1:]]
         plan += [(f"lag{s:+g}", plan[2][1], plan[2][2], s, True) for s in (-lag_ms, lag_ms)]
-        out = []
-        for name, R, T, shift_ms, frozen in plan:
-            r = self.run(None if name == "run" else R, None if name == "run" else T, shift_ms / 1000.0, frozen)
-            out.append((name, R, T, shift_ms, r))
-        return out
+        runs = self.run_many([(None if name == "run" else R, None if name == "run" else T, shift_ms / 1000.0, frozen)
+                              for name, R, T, shift_ms, frozen in plan], jobs)
+        return [(name, R, T, shift_ms, r) for (name, R, T, shift_ms, _), r in zip(plan, runs)]
 
-    def report(self, R_final, T_final) -> str:
+    def report(self, R_final, T_final, jobs: int = 1) -> str:
         import time
         t0 = time.perf_counter()
-        rows = self.sweep(R_final, T_final)
+        rows = self.sweep(R_final, T_final, jobs=jobs)
         wall = time.perf_counter() - t0
         return replay_report_text(self.info(), self.snapshot_bytes, wall, self.assessment.radius, self.assessment.min_neighbors, rows)
 
     def write(self, path: str, R_final=None, T_final=None):
-        """result/assessment_replay.txt; R_final / T_final: the run's final extrinsic. NOTHING when the run did not hand over."""
+        """result/assessment_replay.txt, self.jobs replays at once; R_final / T_final: the run's final extrinsic. NOTHING when the run
+        did not hand over."""
         with open(path, "w") as f:
-            f.write(NOTHING if self.base is None or not self.frames else self.report(R_final, T_final))
+            f.write(NOTHING if self.base is None or not self.frames else self.report(R_final, T_final, self.jobs))
 
     @property
     def lag(self) -> float:
         """The node's total lag at the hand-over, time_lag_IMU_wtr_lidar + timediff_imu_wrt_lidar [s]; a replay's lag shift adds to it."""
         return float(self.base.imu_buffer.timediff) + float(self.res["time_lag_1"]) + float(self.res["time_lag_2"])
 
-    def refine(self, R_final, T_final, max_replays=None) -> dict:
+    def refine(self, R_final, T_final, max_replays=None, jobs: int = 1) -> dict:
         """refine.search with frozen replays as the scorer, from the run's final extrinsic and LI-Init's at shift 0. Returns search's
         dict with, on every trace row, the replay's "result" (the as-run evaluation) and "seconds"; and "wall_s", "lag0" (the lag at the
         hand-over [s]), "time_lag" (the refined total lag [s]), "state" (the best replay's last posterior state, whose extrinsic is the
-        refined one) and "calib" (node.state_calib_values of that state and lag, the arguments of node.calib_result_text)."""
+        refined one) and "calib" (node.state_calib_values of that state and lag, the arguments of node.calib_result_text). jobs: replays
+        at once; the search scores its batches with run_many."""
         import time
 
         from . import refine as rf
         from .node import state_calib_values
         kept = {}
 
-        def score(R, T, shift_s):
-            r = self.run(R, T, shift_s, frozen=True)
-            kept[rf.key(R, T, shift_s)] = (r["result"], r["seconds"], r["states"][-1][1] if r["states"] else None)
-            return r["result"]["mme"]
+        def score_many(cands):
+            runs = self.run_many([(R, T, shift_s, True) for R, T, shift_s in cands], jobs)
+            for (R, T, shift_s), r in zip(cands, runs):
+                kept[rf.key(R, T, shift_s)] = (r["result"], r["seconds"], r["states"][-1][1] if r["states"] else None)
+            return [r["result"]["mme"] for r in runs]
         t0 = time.perf_counter()
-        out = rf.search(score, R_final, T_final, 0.0, rf.MAX_REPLAYS if max_replays is None else max_replays,
-                        R_init=self.res["R_LI"], T_init=self.res["T_LI"])
+        out = rf.search(lambda R, T, shift_s: score_many([(R, T, shift_s)])[0], R_final, T_final, 0.0,
+                        rf.MAX_REPLAYS if max_replays is None else max_replays, R_init=self.res["R_LI"], T_init=self.res["T_LI"],
+                        score_many=score_many)
         out["wall_s"] = time.perf_counter() - t0
         for row in out["trace"]:
             row["result"], row["seconds"], _ = kept[rf.key(row["R"], row["T"], row["shift_ms"] / 1000.0)]
@@ -429,13 +543,13 @@ class Replay:
         return out
 
     def write_refinement(self, path: str, R_final=None, T_final=None, max_replays=None):
-        """result/refinement.txt (refine_report_text); R_final / T_final: the run's final extrinsic. Returns refine's dict, or None,
-        writing NOTHING, when the run did not hand over."""
+        """result/refinement.txt (refine_report_text), self.jobs replays at once; R_final / T_final: the run's final extrinsic. Returns
+        refine's dict, or None, writing NOTHING, when the run did not hand over."""
         if self.base is None or not self.frames:
             with open(path, "w") as f:
                 f.write(NOTHING)
             return None
-        ref = self.refine(R_final, T_final, max_replays)
+        ref = self.refine(R_final, T_final, max_replays, self.jobs)
         with open(path, "w") as f:
             f.write(refine_report_text(self.info(), ref, self.assessment.radius, self.assessment.min_neighbors))
         return ref

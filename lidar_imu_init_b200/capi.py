@@ -96,6 +96,7 @@ SYMBOLS = [
     "liinit_assess_download_placed", "liinit_assess_cloud", "liinit_assess_reserve_timed", "liinit_assess_hold", "liinit_assess_append_timed",
     "liinit_assess_timing_info", "liinit_assess_evaluate_timed", "liinit_assess_clear", "liinit_map_snapshot", "liinit_map_restore",
     "liinit_replay_reserve", "liinit_replay_append", "liinit_replay_info", "liinit_replay_frame", "liinit_replay_stage",
+    "liinit_replay_share", "liinit_replay_unshare",
 ]
 
 
@@ -209,8 +210,10 @@ def set_replay_argtypes(L):
     L.liinit_replay_info.argtypes = [vp, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_longlong)]
     L.liinit_replay_frame.argtypes = [vp, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_float), C.POINTER(C.c_int)]
     L.liinit_replay_stage.argtypes = [vp, C.c_int]
+    L.liinit_replay_share.argtypes = [vp, vp]
+    L.liinit_replay_unshare.argtypes = [vp]
     for s in ("liinit_assess_clear", "liinit_map_snapshot", "liinit_map_restore", "liinit_replay_reserve", "liinit_replay_append",
-              "liinit_replay_info", "liinit_replay_frame", "liinit_replay_stage"):
+              "liinit_replay_info", "liinit_replay_frame", "liinit_replay_stage", "liinit_replay_share", "liinit_replay_unshare"):
         getattr(L, s).restype = C.c_int
 
 
@@ -259,6 +262,9 @@ class LiInitGpu:
     def __init__(self, filter_size_map=0.15, max_map_points=6_000_000, max_scan_points=300_000, device_id=0, brick_cells_log2=0,
                  hash_capacity_log2=0, knn_group_lanes=0, knn_seed_radius_cells=0.0, knn_index=0):
         self.L = load()
+        self.config = dict(filter_size_map=filter_size_map, max_map_points=max_map_points, max_scan_points=max_scan_points, device_id=device_id,
+                           brick_cells_log2=brick_cells_log2, hash_capacity_log2=hash_capacity_log2, knn_group_lanes=knn_group_lanes,
+                           knn_seed_radius_cells=knn_seed_radius_cells, knn_index=knn_index)
         cfg = Config(filter_size_map, max_map_points, max_scan_points, device_id, brick_cells_log2, hash_capacity_log2, knn_group_lanes, knn_seed_radius_cells,
                      knn_index)
         h = C.c_void_p()
@@ -270,10 +276,16 @@ class LiInitGpu:
         self.device_id = device_id
         self._tstream = None   # (stream pointer, torch.cuda.ExternalStream) of the context's stream
 
+    def twin(self):
+        """A new context with this one's configuration (an empty map)."""
+        return type(self)(**self.config)
+
     def close(self):
+        """Destroy the context. A lead whose replay store workers still share is refused (LiInitError) and stays open."""
         if getattr(self, "h", None):
-            self.L.liinit_destroy(self.h)
+            self._ck(self.L.liinit_destroy(self.h))
             self.h = None
+            self._share_lead = None
 
     def __del__(self):
         try:
@@ -798,6 +810,17 @@ class LiInitGpu:
         """Stored sub-frame j becomes the staged raw cloud, as frame_stage left the original."""
         self._ck(self.L.liinit_replay_stage(self.h, int(j)))
         self.raw_n = self.replay_frame(j)["n"]
+
+    def replay_share(self, lead):
+        """Read `lead`'s replay store and map snapshot from now on (liinit_replay_share); this context keeps its own map and
+        assessment store. Keeps a reference to the lead, which cannot be destroyed while this context shares it."""
+        self._ck(self.L.liinit_replay_share(self.h, lead.h))
+        self._share_lead = lead
+        self._snap_raw_n = getattr(lead, "_snap_raw_n", 0)
+
+    def replay_unshare(self):
+        self._ck(self.L.liinit_replay_unshare(self.h))
+        self._share_lead = None
 
     def knn_index(self) -> int:
         """1 = LIINIT_KNN_BRICKS (lockstep groups over whole bricks), 2 = LIINIT_KNN_CELLS (cell directory, thread per point)."""

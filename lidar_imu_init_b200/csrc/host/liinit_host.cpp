@@ -1,8 +1,10 @@
 // liinit_host.cpp -- host side of the drop-in (see liinit_host.h). Everything here is O(24^3) per iteration.
 #include "liinit_host.h"
 
+#include <array>
 #include <cmath>
 #include <cstring>
+#include <deque>
 #include <vector>
 
 namespace {
@@ -490,6 +492,99 @@ int liinit_imu_propagate(liinit_imu* imu, liinit_state* s, const double* smp, in
     std::memcpy(imu->last_imu, sample(n), sizeof(imu->last_imu));   // :381-382
     imu->last_lidar_end_time = pcl_end_time;
     *npose = out;
+    return LIINIT_OK;
+}
+
+int liinit_replay_run(liinit_ctx* h, const liinit_replay_job* job, liinit_state* states, int* frames, int cap, int* n_updates) {
+    if (!h || !job || !n_updates || cap < 0 || (cap > 0 && (!states || !frames)) || job->n_buf < 0 || job->n_samples < 0 || job->n_events < 0 ||
+        (job->n_buf > 0 && !job->buf_rows) || (job->n_samples > 0 && !job->samples) || (job->n_events > 0 && !job->events) || job->max_iteration < 1)
+        return LIINIT_ERR_INVALID;
+    *n_updates = 0;
+    constexpr int W = LIINIT_IMU_SAMPLE_DOUBLES;
+    using Row = std::array<double, W>;
+    liinit_state s = job->state;
+    liinit_imu imu = job->imu;
+    std::deque<Row> rows;   // ImuBuffer.rows
+    for (int i = 0; i < job->n_buf; i++) {
+        Row r;
+        std::memcpy(r.data(), job->buf_rows + (size_t)i * W, sizeof(Row));
+        rows.push_back(r);
+    }
+    double last_stamp = job->last_stamp;
+    int frame_num = job->frame_num, switch_scan = job->switch_scan, next_sample = 0;
+    std::deque<int> pending;
+    std::vector<double> group, poses;
+    for (int e = 0; e < job->n_events; e++) {
+        const int ev = job->events[e];
+        if (ev >= 0) {
+            pending.push_back(ev);
+        } else if (ev == LIINIT_REPLAY_IMU && next_sample < job->n_samples) {
+            // ImuBuffer.push: imu_cbk's time compensation and its loop-back clear (laserMapping.cpp:412-423)
+            const double* x = job->samples + (size_t)next_sample++ * W;
+            Row r;
+            std::memcpy(r.data(), x, sizeof(Row));
+            r[0] = x[0] - job->timediff - job->time_lag;
+            if (r[0] < last_stamp) rows.clear();
+            last_stamp = r[0];
+            rows.push_back(r);
+        } else {
+            return LIINIT_ERR_INVALID;
+        }
+        while (!pending.empty()) {
+            const int j = pending.front();
+            double t_beg;
+            float end_ms;
+            int rc = liinit_replay_frame(h, j, &t_beg, &end_ms, nullptr);
+            if (rc != LIINIT_OK) return rc;
+            const double t_end = t_beg + (double)end_ms / 1000.0;   // lidar_end_time
+            if (rows.empty() || !(last_stamp >= t_end)) break;     // sync_packages waits for an IMU stamp >= lidar_end_time
+            pending.pop_front();
+            // ImuBuffer.pop: the measure group, the buffered samples with stamp <= lidar_end_time (:466-474)
+            group.clear();
+            double imu_time = rows.empty() ? 0.0 : rows.front()[0];
+            while (!rows.empty() && imu_time < t_end) {
+                imu_time = rows.front()[0];
+                if (imu_time > t_end) break;
+                group.insert(group.end(), rows.front().begin(), rows.front().end());
+                rows.pop_front();
+            }
+            const int n = (int)(group.size() / W);
+            // process_raw in LIO mode
+            if (n && !imu.need_init) {
+                poses.resize((size_t)(n + 1) * LIINIT_POSE6D_DOUBLES);
+                int np = 0;
+                rc = liinit_imu_propagate(&imu, &s, group.data(), n, t_beg, (double)end_ms, poses.data(), &np);
+                if (rc != LIINIT_OK) return rc;
+                rc = liinit_replay_stage(h, j);
+                if (rc != LIINIT_OK) return rc;
+                if (np >= 2) {
+                    rc = liinit_raw_undistort_imu(h, poses.data(), np, s.rot_end, s.pos_end, s.offset_R_L_I, s.offset_T_L_I);
+                    if (rc != LIINIT_OK) return rc;
+                }
+            } else if (n) {
+                rc = liinit_imu_switch(&imu, group.data(), n);   // the switch scan: the previous cloud is matched again
+                if (rc != LIINIT_OK) return rc;
+                switch_scan = frame_num;
+            }
+            int n_down = 0, n_add = 0, n_nd = 0;
+            rc = liinit_raw_downsample(h, (float)job->filter_size_surf, &n_down);
+            if (rc != LIINIT_OK) return rc;
+            rc = scan_update(h, &s, job->max_iteration, 1, nullptr, job->frozen != 0);
+            if (rc != LIINIT_OK) return rc;
+            rc = liinit_map_incremental(h, s.rot_end, s.pos_end, s.offset_R_L_I, s.offset_T_L_I, job->filter_size_map, 1, &n_add, &n_nd);
+            if (rc != LIINIT_OK) return rc;
+            frame_num++;
+            if (*n_updates >= cap) return LIINIT_ERR_CAPACITY;
+            states[*n_updates] = s;
+            frames[*n_updates] = j;
+            ++*n_updates;
+            if (switch_scan != frame_num - 1) {
+                int appended = 0;
+                rc = liinit_assess_append(h, s.rot_end, s.pos_end, s.offset_R_L_I, s.offset_T_L_I, &appended);
+                if (rc != LIINIT_OK) return rc;
+            }
+        }
+    }
     return LIINIT_OK;
 }
 

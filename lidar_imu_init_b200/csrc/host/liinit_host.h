@@ -129,6 +129,42 @@ int liinit_imu_switch(liinit_imu* imu, const double* samples, int n);
 int liinit_imu_propagate(liinit_imu* imu, liinit_state* s, const double* samples, int n, double pcl_beg_time, double pcl_end_offset_ms,
                          double* poses, int* npose);
 
+/* ---- the LIO phase of a replay (DESIGN.md section 4d), natively: assess.Replay.run after the hand-over with no Python in between ----
+ * The hand-over itself (the candidate extrinsic and lag, and for a frozen replay the zero extrinsic rows / columns of cov and the zero
+ * extrinsic noise of the IMU processor) is the caller's; the job holds what the loop starts from. Each event is either a stored
+ * sub-frame (its index in the replay store, liinit_replay_*) or LIINIT_REPLAY_IMU, the next of the recorded IMU samples. The loop:
+ *   an IMU sample: imu_cbk's compensation (stamp = t - timediff - time_lag; an older stamp than the last clears the buffer), appended;
+ *   a sub-frame: queued; then, while the oldest queued sub-frame's lidar_end_time = t_beg + end_ms / 1000 has an IMU stamp at or after
+ *   it (sync_packages), its measure group is popped and process_raw's LIO body runs: a group with the IMU processor switched propagates
+ *   (liinit_imu_propagate), stages the sub-frame (liinit_replay_stage) and undistorts it (liinit_raw_undistort_imu, two poses or more);
+ *   a group before the switch switches it (liinit_imu_switch: the switch scan); an empty group does neither. Then liinit_raw_downsample
+ *   (filter_size_surf as float), liinit_scan_update[_frozen] (imu_en), liinit_map_incremental (filter_size_map) and, for every update but
+ *   the switch scan, liinit_assess_append of the staged cloud with the posterior pose and extrinsic.
+ * The map must be ready (the hand-over comes after the LiDAR-only phase built it): the loop never builds one. */
+#define LIINIT_REPLAY_IMU (-1)
+typedef struct liinit_replay_job {
+    liinit_state state;           /* the state after the hand-over */
+    liinit_imu imu;               /* the IMU processor after the hand-over */
+    const double* buf_rows;       /* the IMU buffer after the hand-over: n_buf rows {stamp, gyr xyz, acc xyz}, stamps compensated */
+    const double* samples;        /* the recorded IMU samples as they arrived, n_samples x {t, gyr xyz, acc xyz} */
+    const int* events;            /* n_events: a stored sub-frame index (>= 0) or LIINIT_REPLAY_IMU */
+    double last_stamp;            /* the buffer's last compensated stamp (-inf: none) */
+    double timediff;              /* timediff_imu_wrt_lidar */
+    double time_lag;              /* time_lag_IMU_wtr_lidar, the candidate's */
+    double filter_size_surf;      /* the scan voxel grid's leaf */
+    double filter_size_map;       /* map_incremental's ds */
+    int n_buf, n_samples, n_events;
+    int frame_num;                /* the loop's frame counter at the hand-over */
+    int switch_scan;              /* frame_num of the switch scan; -1: not yet */
+    int max_iteration;
+    int frozen;                   /* liinit_scan_update_frozen: the extrinsic held constant */
+    int reserved;
+} liinit_replay_job;
+/* Runs the loop on h. states[k] / frames[k] (room for cap): the posterior state and the stored sub-frame index of update k, for
+ * *n_updates updates. Returns LIINIT_OK, or the code of the first call that failed (the updates before it are in states / frames);
+ * LIINIT_ERR_INVALID for a bad job (an event past the recorded samples, a negative count), LIINIT_ERR_CAPACITY when cap is too small. */
+int liinit_replay_run(liinit_ctx* h, const liinit_replay_job* job, liinit_state* states, int* frames, int cap, int* n_updates);
+
 /* lasermap_fov_segment (laserMapping.cpp:260-305): keeps a cube_len-sized local map box around the LiDAR and, when the
  * LiDAR comes within MOV_THRESHOLD*det_range of a face, shifts the box and returns the slabs that fell out of it
  * (cub_needrm) -- the boxes to hand to liinit_map_delete_boxes. local_box: {min xyz, max xyz}, state kept by the caller;

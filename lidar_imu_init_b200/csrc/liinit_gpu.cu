@@ -13,6 +13,7 @@
 #include <nccl.h>   // types only: the library is dlopen()ed when a communicator is asked for (no link-time dependency)
 #endif
 
+#include <atomic>
 #include <cmath>
 #include <cstddef>
 #include <cstdio>
@@ -284,6 +285,10 @@ struct Ctx {
         int raw_n = 0;
         bool stage_attr_on = false;
     } snap;
+    // replay sharing (liinit_replay_share): a worker reads its lead's replay store and map snapshot instead of its own; a lead counts
+    // the workers that read its store and snapshot (while any does, neither may change or go away)
+    Ctx* share_lead = nullptr;
+    std::atomic<int> share_workers{0};
 };
 
 #define CU(call)                                                                                     \
@@ -1080,7 +1085,14 @@ int liinit_create(const liinit_config* cfg, liinit_ctx** out) {
 int liinit_destroy(liinit_ctx* h) {
     if (!h) return LIINIT_OK;
     Ctx* c = &h->c;
+    if (c->share_workers.load() > 0)
+        return fail(c, LIINIT_ERR_INVALID, "workers share this context's replay store and map snapshot (liinit_replay_unshare them first)");
     cudaSetDevice(c->device);
+    if (c->share_lead) {
+        cudaStreamSynchronize(c->stream);   // its last reads of the lead's store and snapshot are done
+        c->share_lead->share_workers--;
+        c->share_lead = nullptr;
+    }
     if (c->own_stream) cudaStreamSynchronize(c->own_stream);
     cudaFree(c->M.ent); cudaFree(c->M.brick_slots); cudaFree(c->M.aux); cudaFree(c->M.pool); cudaFree(c->M.pool_top); cudaFree(c->M.touched_list); cudaFree(c->M.cocc); cudaFree(c->M.cdir); cudaFree(c->M.sb_keys); cudaFree(c->M.sb_occ); cudaFree(c->d_ticket);
     cudaFree(c->d_counters); cudaFreeHost(c->h_counters); cudaFreeHost(c->h_pool_top); cudaFree(c->d_stage_raw); cudaFree(c->d_stage_pts);
@@ -2834,6 +2846,17 @@ cudaError_t regrow(T*& p, size_t count) {
     return cudaMalloc(&p, count * sizeof(T));
 }
 
+// the replay store a context reads: its lead's while it shares one (liinit_replay_share), else its own
+const Ctx::Replay& replay_store(const Ctx* c) { return c->share_lead ? c->share_lead->R : c->R; }
+
+// the calls that change a replay store or a map snapshot are refused on a worker and on a lead with workers
+int refuse_shared(Ctx* c, const char* what) {
+    if (c->share_lead) return fail(c, LIINIT_ERR_INVALID, std::string(what) + " on a context that shares a lead's replay store (liinit_replay_unshare it first)");
+    if (c->share_workers.load() > 0)
+        return fail(c, LIINIT_ERR_INVALID, std::string(what) + " on a context whose replay store and map snapshot workers share (liinit_replay_unshare them first)");
+    return LIINIT_OK;
+}
+
 int map_snapshot(Ctx* c, long long* bytes) {
     int r = fetch_counters(c);   // (synchronises: the host mirrors and the counts that size the copies are current)
     if (r) return r;
@@ -2892,7 +2915,7 @@ int map_snapshot(Ctx* c, long long* bytes) {
 }
 
 int map_restore(Ctx* c) {
-    Ctx::Snap& S = c->snap;
+    const Ctx::Snap& S = c->share_lead ? c->share_lead->snap : c->snap;
     if (!S.have) return fail(c, LIINIT_ERR_INVALID, "no map snapshot (liinit_map_snapshot)");
     const size_t slots = c->hash_slots;
     auto d2d = [&](void* dst, const void* src, size_t n) {
@@ -2945,6 +2968,8 @@ int liinit_map_snapshot(liinit_ctx* h, long long* bytes) {
     if (!h) return LIINIT_ERR_INVALID;
     Ctx* c = &h->c;
     if (has_comm(c)) return fail(c, LIINIT_ERR_INVALID, "the map snapshot does not take a communicator (liinit_comm_init)");
+    int r = refuse_shared(c, "liinit_map_snapshot");
+    if (r) return r;
     CU(cudaSetDevice(c->device));
     return map_snapshot(c, bytes);
 }
@@ -2961,6 +2986,8 @@ int liinit_replay_reserve(liinit_ctx* h, long long max_points, int max_frames) {
     Ctx* c = &h->c;
     if (max_points < 1 || max_points > LIINIT_ASSESS_MAX_POINTS) return fail(c, LIINIT_ERR_INVALID, "max_points must be in [1, LIINIT_ASSESS_MAX_POINTS]");
     if (max_frames < 1 || max_frames > LIINIT_ASSESS_MAX_SCANS) return fail(c, LIINIT_ERR_INVALID, "max_frames must be in [1, LIINIT_ASSESS_MAX_SCANS]");
+    int r = refuse_shared(c, "liinit_replay_reserve");
+    if (r) return r;
     CU(cudaSetDevice(c->device));
     CU(cudaStreamSynchronize(c->stream));
     replay_free(c);
@@ -2980,6 +3007,8 @@ int liinit_replay_append(liinit_ctx* h, long long handle, double t_beg, float en
     if (!h) return LIINIT_ERR_INVALID;
     Ctx* c = &h->c;
     if (!appended) return fail(c, LIINIT_ERR_INVALID, "null argument");
+    int r = refuse_shared(c, "liinit_replay_append");
+    if (r) return r;
     Ctx::Replay& R = c->R;
     if (R.cap <= 0) return fail(c, LIINIT_ERR_INVALID, "no replay store (liinit_replay_reserve)");
     int slot = 0;
@@ -3003,18 +3032,20 @@ int liinit_replay_append(liinit_ctx* h, long long handle, double t_beg, float en
 int liinit_replay_info(liinit_ctx* h, int* frames, int* skipped, long long* points) {
     if (!h) return LIINIT_ERR_INVALID;
     Ctx* c = &h->c;
-    if (c->R.cap <= 0) return fail(c, LIINIT_ERR_INVALID, "no replay store (liinit_replay_reserve)");
-    if (frames) *frames = (int)c->R.fr.size();
-    if (skipped) *skipped = c->R.skipped;
-    if (points) *points = c->R.n;
+    const Ctx::Replay& R = replay_store(c);
+    if (R.cap <= 0) return fail(c, LIINIT_ERR_INVALID, "no replay store (liinit_replay_reserve)");
+    if (frames) *frames = (int)R.fr.size();
+    if (skipped) *skipped = R.skipped;
+    if (points) *points = R.n;
     return LIINIT_OK;
 }
 
 int liinit_replay_frame(liinit_ctx* h, int j, double* t_beg, float* end_ms, int* n) {
     if (!h) return LIINIT_ERR_INVALID;
     Ctx* c = &h->c;
-    if (j < 0 || j >= (int)c->R.fr.size()) return fail(c, LIINIT_ERR_INVALID, "no such stored sub-frame");
-    const Ctx::ReplayFrame& f = c->R.fr[j];
+    const Ctx::Replay& R = replay_store(c);
+    if (j < 0 || j >= (int)R.fr.size()) return fail(c, LIINIT_ERR_INVALID, "no such stored sub-frame");
+    const Ctx::ReplayFrame& f = R.fr[j];
     if (t_beg) *t_beg = f.t_beg;
     if (end_ms) *end_ms = f.end_ms;
     if (n) *n = f.n;
@@ -3024,17 +3055,54 @@ int liinit_replay_frame(liinit_ctx* h, int j, double* t_beg, float* end_ms, int*
 int liinit_replay_stage(liinit_ctx* h, int j) {
     if (!h) return LIINIT_ERR_INVALID;
     Ctx* c = &h->c;
-    if (j < 0 || j >= (int)c->R.fr.size()) return fail(c, LIINIT_ERR_INVALID, "no such stored sub-frame");
+    const Ctx::Replay& R = replay_store(c);
+    if (j < 0 || j >= (int)R.fr.size()) return fail(c, LIINIT_ERR_INVALID, "no such stored sub-frame");
     CU(cudaSetDevice(c->device));
-    const Ctx::ReplayFrame& f = c->R.fr[j];
+    const Ctx::ReplayFrame& f = R.fr[j];
     // liinit_frame_stage's copy and attribute kernel, from the store instead of the message slot
-    CU(cudaMemcpyAsync(c->d_stage_pts, c->R.pts + f.lo, (size_t)f.n * sizeof(float4), cudaMemcpyDeviceToDevice, c->stream));
-    k_attr_from_inten<<<nblk(f.n, 256), 256, 0, c->stream>>>(c->R.inten + f.lo, f.n, c->d_stage_attr);
+    CU(cudaMemcpyAsync(c->d_stage_pts, R.pts + f.lo, (size_t)f.n * sizeof(float4), cudaMemcpyDeviceToDevice, c->stream));
+    k_attr_from_inten<<<nblk(f.n, 256), 256, 0, c->stream>>>(R.inten + f.lo, f.n, c->d_stage_attr);
     c->launches++;
     CU(cudaGetLastError());
     c->stage_attr = true;
     c->raw_n = f.n;
     c->stage_seq++;
+    return LIINIT_OK;
+}
+
+int liinit_replay_share(liinit_ctx* worker, liinit_ctx* lead) {
+    if (!worker) return LIINIT_ERR_INVALID;
+    Ctx* c = &worker->c;
+    if (!lead) return fail(c, LIINIT_ERR_INVALID, "null lead");
+    Ctx* L = &lead->c;
+    if (worker == lead) return fail(c, LIINIT_ERR_INVALID, "a context cannot share its own replay store");
+    if (c->device != L->device) return fail(c, LIINIT_ERR_INVALID, "the worker and the lead are on different devices");
+    if (c->hash_slots != L->hash_slots || c->M.bshift != L->M.bshift || c->cells != L->cells || c->M.pool_cap != L->M.pool_cap ||
+        c->stage_pts_cap != L->stage_pts_cap || c->cfg.max_map_points != L->cfg.max_map_points || c->cfg.max_scan_points != L->cfg.max_scan_points ||
+        c->M.ds != L->M.ds)
+        return fail(c, LIINIT_ERR_INVALID, "the worker's configuration differs from the lead's (hash slots, brick cells, cell directory, "
+                                           "capacities or filter_size_map)");
+    if (has_comm(c) || has_comm(L)) return fail(c, LIINIT_ERR_INVALID, "replay sharing does not take a communicator (liinit_comm_init)");
+    if (c->share_lead) return fail(c, LIINIT_ERR_INVALID, "the worker already shares a lead's replay store");
+    if (c->share_workers.load() > 0) return fail(c, LIINIT_ERR_INVALID, "the worker is itself the lead of other workers");
+    if (L->share_lead) return fail(c, LIINIT_ERR_INVALID, "the lead shares another context's replay store");
+    if (!L->snap.have) return fail(c, LIINIT_ERR_INVALID, "the lead has no map snapshot (liinit_map_snapshot)");
+    if (L->R.cap <= 0) return fail(c, LIINIT_ERR_INVALID, "the lead has no replay store (liinit_replay_reserve)");
+    CU(cudaSetDevice(L->device));
+    CU(cudaStreamSynchronize(L->stream));   // the store and the snapshot are complete before any worker's stream reads them
+    c->share_lead = L;
+    L->share_workers++;
+    return LIINIT_OK;
+}
+
+int liinit_replay_unshare(liinit_ctx* worker) {
+    if (!worker) return LIINIT_ERR_INVALID;
+    Ctx* c = &worker->c;
+    if (!c->share_lead) return fail(c, LIINIT_ERR_INVALID, "the context does not share a lead's replay store");
+    CU(cudaSetDevice(c->device));
+    CU(cudaStreamSynchronize(c->stream));   // its reads of the lead's store and snapshot are done
+    c->share_lead->share_workers--;
+    c->share_lead = nullptr;
     return LIINIT_OK;
 }
 

@@ -27,6 +27,15 @@ class Imu(C.Structure):
                 ("mean_acc_norm", C.c_double), ("need_init", C.c_int), ("reserved", C.c_int)]
 
 
+class ReplayJob(C.Structure):
+    """struct liinit_replay_job: where the native LIO loop of a replay starts (csrc/host/liinit_host.h)."""
+    _fields_ = [("state", C.c_double * STATE_DOUBLES), ("imu", Imu), ("buf_rows", C.c_void_p), ("samples", C.c_void_p), ("events", C.c_void_p),
+                ("last_stamp", C.c_double), ("timediff", C.c_double), ("time_lag", C.c_double), ("filter_size_surf", C.c_double),
+                ("filter_size_map", C.c_double), ("n_buf", C.c_int), ("n_samples", C.c_int), ("n_events", C.c_int), ("frame_num", C.c_int),
+                ("switch_scan", C.c_int), ("max_iteration", C.c_int), ("frozen", C.c_int), ("reserved", C.c_int)]
+
+
+REPLAY_IMU = -1          # LIINIT_REPLAY_IMU: an event that is the next recorded IMU sample
 IMU_SAMPLE_DOUBLES = 7   # {stamp, gyr xyz, acc xyz}
 POSE6D_DOUBLES = 22      # {offset_time, acc[3], gyr[3], vel[3], pos[3], rot[9]}
 MAX_IMU_POSES = 4096     # LIINIT_MAX_IMU_POSES (include/liinit_gpu.h)
@@ -67,11 +76,49 @@ def load():
     L.liinit_imu_switch.argtypes = [pimu, _f64, C.c_int]
     L.liinit_imu_propagate.restype = C.c_int
     L.liinit_imu_propagate.argtypes = [pimu, _f64, _f64, C.c_int, C.c_double, C.c_double, _f64, C.POINTER(C.c_int)]
+    set_replay_run_argtypes(L)
     L.liinit_fov_segment.restype = C.c_int
     L.liinit_fov_segment.argtypes = [_f64, C.c_double, C.c_double, np.ctypeslib.ndpointer(dtype=np.float32, flags='C_CONTIGUOUS'), C.POINTER(C.c_int),
                                      np.ctypeslib.ndpointer(dtype=np.float32, flags='C_CONTIGUOUS')]
     _LIB = L
     return L
+
+
+def set_replay_run_argtypes(L):
+    """argtypes of liinit_replay_run on a loaded host library"""
+    L.liinit_replay_run.restype = C.c_int
+    L.liinit_replay_run.argtypes = [C.c_void_p, C.POINTER(ReplayJob), _f64, np.ctypeslib.ndpointer(dtype=np.int32, flags="C_CONTIGUOUS"), C.c_int,
+                                    C.POINTER(C.c_int)]
+
+
+def replay_run(gpu, odom, samples, events, lib=None):
+    """liinit_replay_run on gpu's context from a handed-over LidarOdometry `odom` (its state, IMU processor, IMU buffer and loop
+    settings): samples [k, 7] the recorded IMU samples {t, gyr, acc} as they arrived, events int32 (a stored sub-frame index or
+    REPLAY_IMU). lib: the host library to run it in (default: this package's). Returns [(stored sub-frame index, posterior state)] of
+    every update; raises capi.LiInitError with the context's message when a call failed."""
+    L = load() if lib is None else lib
+    samples = np.ascontiguousarray(samples, np.float64).reshape(-1, IMU_SAMPLE_DOUBLES)
+    events = np.ascontiguousarray(events, np.int32)
+    ib = odom.imu_buffer
+    buf = np.ascontiguousarray(np.array(list(ib.rows), np.float64).reshape(-1, IMU_SAMPLE_DOUBLES))
+    job = ReplayJob()
+    job.state[:] = [float(x) for x in np.asarray(odom.state, np.float64)]
+    job.imu = Imu.from_buffer_copy(odom.imu_proc.m)
+    job.buf_rows, job.samples, job.events = buf.ctypes.data, samples.ctypes.data, events.ctypes.data
+    job.last_stamp, job.timediff, job.time_lag = float(ib.last_stamp), float(ib.timediff), float(ib.time_lag)
+    job.filter_size_surf, job.filter_size_map = float(odom.filter_size_surf), float(odom.ds)
+    job.n_buf, job.n_samples, job.n_events = len(buf), len(samples), len(events)
+    job.frame_num = int(odom.frame_num)
+    job.switch_scan = -1 if odom.switch_scan is None else int(odom.switch_scan)
+    job.max_iteration, job.frozen = int(odom.max_iteration), int(bool(odom.frozen))
+    cap = int(np.count_nonzero(events >= 0))
+    states = np.zeros((max(cap, 1), STATE_DOUBLES))
+    frames = np.zeros(max(cap, 1), np.int32)
+    n = C.c_int(0)
+    rc = L.liinit_replay_run(gpu.h, C.byref(job), states.reshape(-1), frames, cap, C.byref(n))
+    if rc != 0:
+        raise capi.LiInitError(rc, "liinit_replay_run: " + (gpu.L.liinit_last_error(gpu.h) or b"").decode())
+    return [(int(frames[k]), states[k].copy()) for k in range(n.value)]
 
 
 def state_init():

@@ -15,6 +15,11 @@ tests. It starts from the lower-scoring of the run's final extrinsic and LI-Init
 Every evaluation is cached by the exact bytes of (R, T, shift_s): a revisited candidate is not scored again, and every score is one row
 of the trace. The candidate kept at every point is the lowest MME so far, the first of equals, so an axis along which the MME does not
 change keeps its value. The search stops early when max_replays scores are spent.
+
+With score_many(candidates) -> [MME], the candidates the search needs together are scored as one batch: the start pair, stage 1's
+first pair, each golden-section opening pair and each compass round (at most 12). A batch drops cached candidates and repeated keys and
+is cut at the remaining budget; its rows are appended, and the best row updated, in the order the one-at-a-time search scores them.
+With a deterministic scorer the trace, the result, the status and the axes are those of the one-at-a-time search at the same budget.
 """
 from __future__ import annotations
 
@@ -61,9 +66,9 @@ def moves(R, T, dtheta_deg, dt) -> list:
     return out
 
 
-def search(score, R0, T0, shift0=0.0, max_replays=MAX_REPLAYS, R_init=None, T_init=None) -> dict:
+def search(score, R0, T0, shift0=0.0, max_replays=MAX_REPLAYS, R_init=None, T_init=None, score_many=None) -> dict:
     """The refinement; R0 / T0: the run's final extrinsic, R_init / T_init (optional): LI-Init's; shift0: the lag shift both start at
-    [s]. Returns {"R", "T", "shift_ms", "shift_s", "mme": the best candidate; "start": "final" or "li-init"; "status": "converged" or
+    [s]; score_many (optional): scores a list of (R, T, shift_s) at once, for the search's batches. Returns {"R", "T", "shift_ms", "shift_s", "mme": the best candidate; "start": "final" or "li-init"; "status": "converged" or
     "budget"; "at_edge": stage 1's minimum lay at the +-LAG_CAP_MS cap; "trace": [{"stage", "R", "T", "shift_ms", "mme"}] in evaluation
     order; "best": the index of the best row; "steps": the compass steps (dtheta [deg], dt [m]) it ended with; "axes": {"rot_x": (step,
     MME(+step) - MME, MME(-step) - MME), ...} around the best candidate, NaN where that neighbour was not scored}."""
@@ -73,18 +78,32 @@ def search(score, R0, T0, shift0=0.0, max_replays=MAX_REPLAYS, R_init=None, T_in
     st = dict(best=None, steps=(DTHETA_DEG, DT_M), at_edge=False, start=None)
 
     def f(stage, R, T, ms):
-        R, T = np.array(R, np.float64).reshape(3, 3), np.array(T, np.float64).reshape(3)
-        k = key(R, T, ms / 1000.0)
-        if k in cache:
-            return cache[k]
-        if len(trace) >= max_replays:
-            raise _Budget
-        m = float(score(R, T, ms / 1000.0))
-        cache[k] = m
-        trace.append(dict(stage=stage, R=R, T=T, shift_ms=ms, mme=m))
-        if st["best"] is None or _lower(m, trace[st["best"]]["mme"]):
-            st["best"] = len(trace) - 1
-        return m
+        return fmany([(stage, R, T, ms)])[0]
+
+    def fmany(items):
+        """[MME] of [(stage, R, T, shift_ms)], scored as f would one after the other: the uncached keys, each once, up to the budget,
+        in one call of score_many"""
+        items = [(stage, np.array(R, np.float64).reshape(3, 3), np.array(T, np.float64).reshape(3), ms) for stage, R, T, ms in items]
+        keys = [key(R, T, ms / 1000.0) for _, R, T, ms in items]
+        todo = list(dict.fromkeys(k for k in keys if k not in cache))[:max(max_replays - len(trace), 0)]
+        if todo:
+            at = {k: i for i, k in reversed(list(enumerate(keys)))}
+            cands = [(items[at[k]][1], items[at[k]][2], items[at[k]][3] / 1000.0) for k in todo]
+            got = score_many(cands) if score_many is not None and len(cands) > 1 else [score(*c) for c in cands]
+            fresh = dict(zip(todo, (float(m) for m in got)))
+        else:
+            fresh = {}
+        out = []
+        for (stage, R, T, ms), k in zip(items, keys):
+            if k not in cache:
+                if k not in fresh:
+                    raise _Budget
+                m = cache[k] = fresh[k]
+                trace.append(dict(stage=stage, R=R, T=T, shift_ms=ms, mme=m))
+                if st["best"] is None or _lower(m, trace[st["best"]]["mme"]):
+                    st["best"] = len(trace) - 1
+            out.append(cache[k])
+        return out
 
     def centre():
         b = trace[st["best"]]
@@ -96,7 +115,7 @@ def search(score, R0, T0, shift0=0.0, max_replays=MAX_REPLAYS, R_init=None, T_in
         """golden-section search of the lag on [a, b] at the best extrinsic"""
         R, T, _ = centre()
         x1, x2 = b - _GOLD * (b - a), a + _GOLD * (b - a)
-        f1, f2 = f(stage, R, T, x1), f(stage, R, T, x2)
+        f1, f2 = fmany([(stage, R, T, x1), (stage, R, T, x2)])
         while True:
             if not _lower(f2, f1):
                 b, x2, f2 = x2, x1, f1
@@ -116,8 +135,7 @@ def search(score, R0, T0, shift0=0.0, max_replays=MAX_REPLAYS, R_init=None, T_in
             st["steps"] = (dth, dt)
             before = st["best"]
             R, T, ms = centre()
-            for _, _, Rm, Tm in moves(R, T, dth, dt):
-                f(stage, Rm, Tm, ms)
+            fmany([(stage, Rm, Tm, ms) for _, _, Rm, Tm in moves(R, T, dth, dt)])
             if st["best"] != before:
                 continue
             if dth <= DTHETA_MIN_DEG and dt <= DT_MIN_M:
@@ -127,14 +145,13 @@ def search(score, R0, T0, shift0=0.0, max_replays=MAX_REPLAYS, R_init=None, T_in
     status = "converged"
     try:
         c = shift0 * 1000.0
-        f("final", R0, T0, c)
-        st["start"] = "final"
-        if R_init is not None:
-            f("li-init", R_init, T_init, c)
-            st["start"] = trace[st["best"]]["stage"]
+        st["start"] = "final"      # (max_replays >= 1: the final extrinsic is always scored)
+        fmany([("final", R0, T0, c)] + ([("li-init", R_init, T_init, c)] if R_init is not None else []))
+        st["start"] = trace[st["best"]]["stage"]
         # stage 1: bracket downhill in LAG_STEP_MS steps, then golden-section search
         R, T, _ = centre()
-        fc, fp, fm = trace[st["best"]]["mme"], f("lag", R, T, c + LAG_STEP_MS), f("lag", R, T, c - LAG_STEP_MS)
+        fc = trace[st["best"]]["mme"]
+        fp, fm = fmany([("lag", R, T, c + LAG_STEP_MS), ("lag", R, T, c - LAG_STEP_MS)])
         if not (_lower(fp, fc) or _lower(fm, fc)):
             golden("lag", c - LAG_STEP_MS, c + LAG_STEP_MS)
         else:

@@ -91,7 +91,22 @@ def parse_args(argv=None):
     ap.add_argument("--refine", action="store_true", help="search, by LIO replay, for the lag and extrinsic whose map is sharpest and "
                     "write the refined calibration: DIR/result/refinement.txt (records the replay like --assess-replay)")
     ap.add_argument("--refine-max-replays", metavar="N", help=f"replays the refinement may spend (default {refinemod.MAX_REPLAYS})")
+    ap.add_argument("--replay-jobs", metavar="K", help="replays of --assess-replay and --refine run at once, each on its own device "
+                    "context sharing the recorded replay (default 1)")
     return ap.parse_args(argv)
+
+
+def replay_jobs(args) -> int:
+    """--replay-jobs as a positive integer (1 when it is not given)."""
+    if args.replay_jobs is None:
+        return 1
+    try:
+        n = int(args.replay_jobs)
+    except ValueError:
+        n = 0
+    if n < 1:
+        raise cfgmod.ConfigError(f"--replay-jobs {args.replay_jobs!r}: must be a positive integer")
+    return n
 
 
 def refine_max_replays(args) -> int:
@@ -150,6 +165,7 @@ def main(argv=None, on_node=None) -> int:
         if replaying and args.assess_replay_max_points < 1:
             raise cfgmod.ConfigError(f"--assess-replay-max-points {args.assess_replay_max_points}: must be positive")
         max_replays = refine_max_replays(args) if args.refine else None
+        jobs = replay_jobs(args)
         with rosbag2.open_bag(args.bag) as bag:
             bag.check_topics(cfgmod.wanted_topics(cfg, bag.format))
             if args.record:
@@ -166,6 +182,7 @@ def main(argv=None, on_node=None) -> int:
                 node.odom.assess_hold = args.assess_time
             if replaying:
                 node.replay = node.odom.replay = assessmod.Replay(node.odom.g, node.assess, args.assess_replay_max_points)
+                node.replay.jobs = jobs
             if on_node is not None:
                 on_node(node)
             t0 = time.perf_counter()
@@ -195,7 +212,7 @@ def main(argv=None, on_node=None) -> int:
             path = os.path.join(args.out, "result", "assessment_replay.txt")
             _, _, R_final, T_final = host.state_pose(node.odom.state)
             node.replay.write(path, R_final, T_final)
-            log.info(f"replay assessment written to {path} in {time.perf_counter() - t0:.1f} s")
+            log.info(f"replay assessment written to {path} in {time.perf_counter() - t0:.1f} s ({jobs} replay job{'s' if jobs > 1 else ''})")
         if args.refine:
             # (after --assess-replay: every replay refills the assessment store)
             path = os.path.join(args.out, "result", "refinement.txt")
@@ -204,7 +221,9 @@ def main(argv=None, on_node=None) -> int:
             if ref is None:
                 log.warn(f"{path}: {assessmod.NOTHING.strip()}")
             else:
-                log.info(refine_summary(path, ref))
+                log.info(refine_summary(path, ref, jobs))
+        if replaying:
+            node.replay.close()
         node.odom.g.close()
         log.info(f"{node.updates} updates in {wall:.1f} s; {node.odom.dropped_subframes} sub-frames dropped")
         return 0
@@ -218,12 +237,14 @@ def main(argv=None, on_node=None) -> int:
         raise
 
 
-def refine_summary(path: str, ref: dict) -> str:
-    """The refinement's summary line: the lag, extrinsic change and MME from the start candidate to the refined one."""
+def refine_summary(path: str, ref: dict, jobs: int = 1) -> str:
+    """The refinement's summary line: the replays and jobs, the lag, extrinsic change and MME from the start candidate to the refined
+    one."""
     import numpy as np
     s = ref["trace"][[r["stage"] for r in ref["trace"]].index(ref["start"])]
     c = np.clip((np.trace(ref["R"] @ s["R"].T) - 1.0) / 2.0, -1.0, 1.0)
-    return (f"refinement written to {path}: {len(ref['trace'])} replays in {ref['wall_s']:.1f} s ({ref['status']}); lag "
+    return (f"refinement written to {path}: {len(ref['trace'])} replays in {ref['wall_s']:.1f} s ({ref['status']}, {jobs} replay "
+            f"job{'s' if jobs > 1 else ''}); lag "
             f"{ref['lag0'] * 1000.0:.3f} -> {ref['time_lag'] * 1000.0:.3f} ms; from {ref['start']}: rotation {np.degrees(np.arccos(c)):.4f} deg, "
             f"translation {np.linalg.norm(ref['T'] - s['T']) * 1000.0:.2f} mm; MME {s['mme']:.6f} -> {ref['mme']:.6f}")
 
