@@ -438,40 +438,7 @@ class Replay:
         the candidates in list order. Returns run()'s dicts in list order; "seconds" is each replay's own wall time. native (default:
         jobs > 1): the native loop (run_native), else run() on this context. threads (default self.threads, else one per context): 1
         drives the contexts in turn from the calling thread."""
-        import threading
-        cands = list(cands)
-        ctxs = self.pool(jobs)
-        if not (jobs > 1 if native is None else native):
-            return [self.run(*c) for c in cands]
-        threads = self.threads if threads is None else threads
-        threads = len(ctxs) if threads is None else min(int(threads), len(ctxs))
-        out = [None] * len(cands)
-        if threads <= 1 or len(cands) <= 1:
-            for i, c in enumerate(cands):
-                out[i] = self.run_native(*c, g=ctxs[i % len(ctxs)])
-            return out
-        lock, nxt, errors = threading.Lock(), iter(range(len(cands))), []
-
-        def work(g):
-            while True:
-                with lock:
-                    i = None if errors else next(nxt, None)
-                if i is None:
-                    return
-                try:
-                    out[i] = self.run_native(*cands[i], g=g)
-                except BaseException as e:
-                    with lock:
-                        errors.append((i, e))
-                    return
-        ts = [threading.Thread(target=work, args=(g,)) for g in ctxs[:threads]]
-        for t in ts:
-            t.start()
-        for t in ts:
-            t.join()
-        if errors:
-            raise min(errors, key=lambda x: x[0])[1]
-        return out
+        return run_across([(self, c) for c in cands], jobs, threads, native)
 
     def close(self):
         """Destroy the workers (the context they share can then be destroyed)."""
@@ -553,6 +520,58 @@ class Replay:
         with open(path, "w") as f:
             f.write(refine_report_text(self.info(), ref, self.assessment.radius, self.assessment.min_neighbors))
         return ref
+
+
+def run_across(tasks, jobs: int = 1, threads=None, native=None) -> list:
+    """Replays of one or more recordings at once: tasks [(replay, (R_LI, T_LI, lag_shift [s], frozen))]. Every replay named runs its
+    own tasks on the contexts of its pool(jobs), one thread per context, the threads of every replay at once, each taking its replay's
+    tasks in list order. Returns Replay.run's dicts in task order; an error of a task stops the batch and the first such error by task
+    order is raised. native (default: more than one context in all): the native loop (run_native), else Replay.run. threads (default
+    the smallest Replay.threads set, else one per context): 1 drives the contexts in turn from the calling thread, each replay's tasks on
+    its contexts round robin."""
+    import threading
+    tasks = list(tasks)
+    replays = list(dict.fromkeys(rp for rp, _ in tasks))
+    pools = {rp: rp.pool(jobs) for rp in replays}
+    nctx = sum(len(p) for p in pools.values())
+    if not (nctx > 1 if native is None else native):
+        return [rp.run(*c) for rp, c in tasks]
+    if threads is None:
+        threads = min((rp.threads for rp in replays if rp.threads is not None), default=None)
+    out = [None] * len(tasks)
+    if (threads is not None and int(threads) <= 1) or len(tasks) <= 1:
+        seen = dict.fromkeys(replays, 0)
+        for i, (rp, c) in enumerate(tasks):
+            out[i] = rp.run_native(*c, g=pools[rp][seen[rp] % len(pools[rp])])
+            seen[rp] += 1
+        return out
+    # contexts round robin across the replays, so that a thread limit below the contexts still serves every replay
+    ctxs = [(rp, p[k]) for k in range(max(len(p) for p in pools.values())) for rp, p in pools.items() if k < len(p)]
+    if threads is not None:
+        ctxs = ctxs[:max(int(threads), len(replays))]
+    lock, errors = threading.Lock(), []
+    nxt = {rp: iter([i for i, (r, _) in enumerate(tasks) if r is rp]) for rp in replays}
+
+    def work(rp, g):
+        while True:
+            with lock:
+                i = None if errors else next(nxt[rp], None)
+            if i is None:
+                return
+            try:
+                out[i] = rp.run_native(*tasks[i][1], g=g)
+            except BaseException as e:
+                with lock:
+                    errors.append((i, e))
+                return
+    ts = [threading.Thread(target=work, args=c) for c in ctxs]
+    for t in ts:
+        t.start()
+    for t in ts:
+        t.join()
+    if errors:
+        raise min(errors, key=lambda x: x[0])[1]
+    return out
 
 
 def host_pose(state):
@@ -675,3 +694,89 @@ def parse_refine_report(text: str) -> dict:
         f = line.split()
         axes[f[0]] = (f[1], float(f[2]), float(f[3]), float(f[4]))
     return {"header": header, "rows": rows, "axes": axes, "result": result}
+
+
+_JOINT_INT = ("recordings", "candidates", "replays", "jobs", "at_edge", "n_min", "subframes", "skipped")
+
+
+def _euler_t(R, T) -> str:
+    from .node import rot_to_euler
+    e = np.degrees(rot_to_euler(np.asarray(R, float).reshape(3, 3)))
+    T = np.asarray(T, float).reshape(3)
+    return "%.6f,%.6f,%.6f %.6f,%.6f,%.6f" % (e[0], e[1], e[2], T[0], T[1], T[2])
+
+
+def joint_report_text(recs: list, ref: dict, radius: float, min_neighbors: int) -> str:
+    """result/refinement_joint.txt of joint.refine_replays' dict. recs: per recording {"bag", "subframes", "skipped", "lag" (its total lag
+    at the hand-over [s]), "R_init", "T_init" (LI-Init's result), "R_final", "T_final" (the run's final extrinsic)}. A header line of key
+    value pairs (the recordings, candidates and replays, the start, the wall time, converged or budget, at_edge, L0, the refined shift and
+    total lag, the score's radius and n_min); one `rec` line per recording (sub-frames, skipped, its lag, LI-Init's and the final
+    extrinsic as roll,pitch,yaw [deg] and x,y,z [m], then the bag to the end of the line); a column line and one fixed-column row per
+    candidate in evaluation order (its stage, the candidate, its total lag, the joint MME and the recordings' MMEs); one line per axis for
+    the joint score (`joint`) and per recording (`rec<b>`): verdict, final step, the + and - neighbour differences; then `Refined
+    result:` and, per recording, `Recording <b>:` and node.calib_result_text of its replay of the refined candidate."""
+    from .node import calib_result_text, rot_to_euler
+    from .refine import axis_verdict
+    B = len(recs)
+    lines = [f"recordings {B} candidates {len(ref['trace'])} replays {len(ref['trace']) * B} start {ref['start']} "
+             f"wall_s {ref['wall_s']:.6f} status {ref['status']} at_edge {int(ref['at_edge'])} lag0_ms {ref['lag0'] * 1000.0:.6f} "
+             f"shift_ms {ref['shift_ms']:.6f} lag_ms {ref['time_lag'] * 1000.0:.6f} radius {radius:.6f} n_min {min_neighbors}"]
+    for b, r in enumerate(recs):
+        lines.append(f"rec {b} subframes {r['subframes']} skipped {r['skipped']} lag_ms {r['lag'] * 1000.0:.6f} "
+                     f"li_init {_euler_t(r['R_init'], r['T_init'])} final {_euler_t(r['R_final'], r['T_final'])} bag {r['bag']}")
+    lines.append("%-10s %11s %11s %11s %10s %10s %10s %11s %15s" % ("stage", "roll_deg", "pitch_deg", "yaw_deg", "t_x", "t_y", "t_z", "lag_ms",
+                                                                 "mme") + "".join(" %15s" % f"mme_{b}" for b in range(B)))
+    for r in ref["trace"]:
+        e, T = np.degrees(rot_to_euler(r["R"])), r["T"]
+        lines.append("%-10s %11.6f %11.6f %11.6f %10.6f %10.6f %10.6f %11.6f %15.9f" % (r["stage"], e[0], e[1], e[2], T[0], T[1], T[2],
+                                                                                   r["lag"] * 1000.0, r["mme"])
+                     + "".join(" %15.9f" % m for m in r["mmes"]))
+    for who, axes in [("joint", ref["axes"])] + [(f"rec{b}", a) for b, a in enumerate(ref["axes_rec"])]:
+        for axis, (step, dp, dm) in axes.items():
+            lines.append("%-6s %-7s %-11s %12.6f %15.9f %15.9f" % (who, axis, axis_verdict(dp, dm), step, dp, dm))
+    blocks = "".join(f"Recording {b}:\n" + calib_result_text(**c) for b, c in enumerate(ref["calibs"]))
+    return "\n".join(lines) + "\n" + REFINED + "\n" + blocks
+
+
+def parse_joint_report(text: str) -> dict:
+    """The inverse of joint_report_text: {"header": {...}, "recs": [{"subframes", "skipped", "lag_ms", "li_init", "final" (each
+    (roll, pitch, yaw, x, y, z)), "bag"}], "rows": [{"stage", ..., "mme", "mmes": [...]}] in evaluation order, "axes": {"joint" or b:
+    {axis: (verdict, step, d_plus, d_minus)}}, "result": [the calib_result_text block of each recording]}."""
+    import re
+    head, result = text.split("\n" + REFINED + "\n", 1)
+    ls = head.splitlines()
+
+    def val(x):
+        for t in (int, float):
+            try:
+                return t(x)
+            except ValueError:
+                pass
+        return x
+    h = ls[0].split()
+    header = {h[i]: val(h[i + 1]) for i in range(0, len(h), 2)}
+    B, n = header["recordings"], header["candidates"]
+    recs = []
+    for line in ls[1:1 + B]:
+        kv, bag = line.split(" bag ", 1)
+        f = kv.split()
+        assert f[0] == "rec" and int(f[1]) == len(recs), line
+        r = {f[i]: val(f[i + 1]) for i in (2, 4, 6)}
+        r["li_init"] = tuple(float(x) for x in (f[9] + "," + f[10]).split(","))
+        r["final"] = tuple(float(x) for x in (f[12] + "," + f[13]).split(","))
+        r["bag"] = bag
+        recs.append(r)
+    cols = ls[1 + B].split()
+    rows = []
+    for line in ls[2 + B:2 + B + n]:
+        f = line.split()
+        row = {c: (x if c == "stage" else float(x)) for c, x in zip(cols[:9], f[:9])}
+        row["mmes"] = [float(x) for x in f[9:]]
+        rows.append(row)
+    axes = {}
+    for line in ls[2 + B + n:]:
+        f = line.split()
+        who = "joint" if f[0] == "joint" else int(f[0][3:])
+        axes.setdefault(who, {})[f[1]] = (f[2], float(f[3]), float(f[4]), float(f[5]))
+    blocks = re.split(r"^Recording \d+:\n", result, flags=re.M)[1:]
+    return {"header": header, "recs": recs, "rows": rows, "axes": axes, "result": blocks}

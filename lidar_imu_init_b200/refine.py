@@ -20,6 +20,9 @@ With score_many(candidates) -> [MME], the candidates the search needs together a
 first pair, each golden-section opening pair and each compass round (at most 12). A batch drops cached candidates and repeated keys and
 is cut at the remaining budget; its rows are appended, and the best row updated, in the order the one-at-a-time search scores them.
 With a deterministic scorer the trace, the result, the status and the axes are those of the one-at-a-time search at the same budget.
+
+With starts=[(label, R, T), ...] the search starts from the lowest of those, scored as one batch at shift0, instead of the (final,
+LI-Init) pair: joint.py starts from every recording's pair.
 """
 from __future__ import annotations
 
@@ -66,9 +69,11 @@ def moves(R, T, dtheta_deg, dt) -> list:
     return out
 
 
-def search(score, R0, T0, shift0=0.0, max_replays=MAX_REPLAYS, R_init=None, T_init=None, score_many=None) -> dict:
+def search(score, R0, T0, shift0=0.0, max_replays=MAX_REPLAYS, R_init=None, T_init=None, score_many=None, starts=None) -> dict:
     """The refinement; R0 / T0: the run's final extrinsic, R_init / T_init (optional): LI-Init's; shift0: the lag shift both start at
-    [s]; score_many (optional): scores a list of (R, T, shift_s) at once, for the search's batches. Returns {"R", "T", "shift_ms", "shift_s", "mme": the best candidate; "start": "final" or "li-init"; "status": "converged" or
+    [s]; score_many (optional): scores a list of (R, T, shift_s) at once, for the search's batches; starts (optional): [(label, R, T)]
+    scored as one batch at shift0 in place of the (final, li-init) pair, R0 / T0 and R_init / T_init then unused. Returns {"R", "T",
+    "shift_ms", "shift_s", "mme": the best candidate; "start": "final" or "li-init" (the label of a start); "status": "converged" or
     "budget"; "at_edge": stage 1's minimum lay at the +-LAG_CAP_MS cap; "trace": [{"stage", "R", "T", "shift_ms", "mme"}] in evaluation
     order; "best": the index of the best row; "steps": the compass steps (dtheta [deg], dt [m]) it ended with; "axes": {"rot_x": (step,
     MME(+step) - MME, MME(-step) - MME), ...} around the best candidate, NaN where that neighbour was not scored}."""
@@ -145,8 +150,10 @@ def search(score, R0, T0, shift0=0.0, max_replays=MAX_REPLAYS, R_init=None, T_in
     status = "converged"
     try:
         c = shift0 * 1000.0
-        st["start"] = "final"      # (max_replays >= 1: the final extrinsic is always scored)
-        fmany([("final", R0, T0, c)] + ([("li-init", R_init, T_init, c)] if R_init is not None else []))
+        if starts is None:
+            starts = [("final", R0, T0)] + ([("li-init", R_init, T_init)] if R_init is not None else [])
+        st["start"] = starts[0][0]      # (max_replays >= 1: the first start is always scored)
+        fmany([(label, R, T, c) for label, R, T in starts])
         st["start"] = trace[st["best"]]["stage"]
         # stage 1: bracket downhill in LAG_STEP_MS steps, then golden-section search
         R, T, _ = centre()

@@ -144,12 +144,12 @@ def make_node(args, cfg, log):
     return Node(cfg, odom, args.out, log)
 
 
-def main(argv=None, on_node=None) -> int:
-    """The command line; on_node(node), when given, is called with the Node before the bag is played (for tools and tests)."""
-    from . import calib, capi, host
-    from .node import Log, Recorder
-    args = parse_args(argv)
-    log = Log(quiet=args.quiet)
+def play(args, log, on_node=None, jobs: int = 1):
+    """Plays args.bag through a new Node with what args asks it to store (--assess*, --refine, --record, --debug-logs) and closes the
+    node, which writes its result files. Returns (node, wall seconds of the bag): the node's context, assessment store and replay stay
+    open for the caller to use and close. on_node(node), when given, is called before the bag is played; jobs: the replay's jobs of
+    Replay.write and write_refinement. On an error the node and the recording are closed and the error is raised."""
+    from .node import Recorder
     node = writer = None
     try:
         cfg = cfgmod.load(args.config, args.param)
@@ -164,8 +164,6 @@ def main(argv=None, on_node=None) -> int:
             raise cfgmod.ConfigError(f"--assess-max-points {args.assess_max_points}: must be positive")
         if replaying and args.assess_replay_max_points < 1:
             raise cfgmod.ConfigError(f"--assess-replay-max-points {args.assess_replay_max_points}: must be positive")
-        max_replays = refine_max_replays(args) if args.refine else None
-        jobs = replay_jobs(args)
         with rosbag2.open_bag(args.bag) as bag:
             bag.check_topics(cfgmod.wanted_topics(cfg, bag.format))
             if args.record:
@@ -189,6 +187,24 @@ def main(argv=None, on_node=None) -> int:
             node.run(bag)
             wall = time.perf_counter() - t0
         node.close()
+        return node, wall
+    except BaseException:
+        # an interrupted run (Ctrl-C) still closes its files and its recording, so the bag it leaves is complete
+        _abort(node, writer)
+        raise
+
+
+def main(argv=None, on_node=None) -> int:
+    """The command line; on_node(node), when given, is called with the Node before the bag is played (for tools and tests)."""
+    from . import host
+    from .node import Log
+    args = parse_args(argv)
+    log = Log(quiet=args.quiet)
+    try:
+        max_replays = refine_max_replays(args) if args.refine else None
+        jobs = replay_jobs(args)
+        replaying = args.assess_replay or args.refine
+        node, wall = play(args, log, on_node, jobs)      # (closed: the error paths below have nothing left to close)
         if args.assess:
             t0 = time.perf_counter()
             node.assess.write(os.path.join(args.out, "result", "assessment.txt"))
@@ -227,14 +243,15 @@ def main(argv=None, on_node=None) -> int:
         node.odom.g.close()
         log.info(f"{node.updates} updates in {wall:.1f} s; {node.odom.dropped_subframes} sub-frames dropped")
         return 0
-    except (cfgmod.ConfigError, rosbag.BagError, rosmsg.MsgError, capi.LiInitError, calib.CalibError, assessmod.ReplayError, OSError) as e:
-        _abort(node, writer)
+    except errors() as e:
         sys.stderr.write(f"error: {e}\n")
         return 1
-    except BaseException:
-        # an interrupted run (Ctrl-C) still closes its files and its recording, so the bag it leaves is complete
-        _abort(node, writer)
-        raise
+
+
+def errors() -> tuple:
+    """The errors the command line reports with a message and exit code 1."""
+    from . import calib, capi
+    return cfgmod.ConfigError, rosbag.BagError, rosmsg.MsgError, capi.LiInitError, calib.CalibError, assessmod.ReplayError, OSError
 
 
 def refine_summary(path: str, ref: dict, jobs: int = 1) -> str:
