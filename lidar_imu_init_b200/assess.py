@@ -521,6 +521,38 @@ class Replay:
             f.write(refine_report_text(self.info(), ref, self.assessment.radius, self.assessment.min_neighbors))
         return ref
 
+    def profile(self, ref, jobs: int = 1, steps=None) -> dict:
+        """profiles.profile around refine's result `ref` (its R, T and shift; its MME is the centre's, not replayed again), with frozen
+        replays as the scorer, all at once on the contexts of pool(jobs). Returns profile's dict with, on every row, the replay's
+        "result" and "seconds"; and "wall_s", "jobs", "replays" and "status" (the refinement's)."""
+        import time
+
+        from . import profiles as pf
+        kept = []
+
+        def score_many(cands):
+            kept[:] = self.run_many([(R, T, s, True) for R, T, s in cands], jobs)
+            return [r["result"]["mme"] for r in kept]
+        t0 = time.perf_counter()
+        out = pf.profile(score_many, ref["R"], ref["T"], ref["shift_s"], ref["mme"], pf.STEPS if steps is None else steps, lag0=self.lag)
+        out["wall_s"] = time.perf_counter() - t0
+        for row, r in zip(out["rows"], kept):
+            row["result"], row["seconds"] = r["result"], r["seconds"]
+        out.update(jobs=jobs, replays=len(out["rows"]), status=ref["status"])
+        return out
+
+    def write_profile(self, path: str, ref, steps=None):
+        """result/profile.txt (profile_report_text) around refine's result `ref`, self.jobs replays at once. Returns profile's dict, or
+        None, writing NOTHING, when there is no refinement (ref None: the run did not hand over)."""
+        if ref is None:
+            with open(path, "w") as f:
+                f.write(NOTHING)
+            return None
+        prof = self.profile(ref, self.jobs, steps)
+        with open(path, "w") as f:
+            f.write(profile_report_text(prof))
+        return prof
+
 
 def run_across(tasks, jobs: int = 1, threads=None, native=None) -> list:
     """Replays of one or more recordings at once: tasks [(replay, (R_LI, T_LI, lag_shift [s], frozen))]. Every replay named runs its
@@ -780,3 +812,87 @@ def parse_joint_report(text: str) -> dict:
         axes.setdefault(who, {})[f[1]] = (f[2], float(f[3]), float(f[4]), float(f[5]))
     blocks = re.split(r"^Recording \d+:\n", result, flags=re.M)[1:]
     return {"header": header, "recs": recs, "rows": rows, "axes": axes, "result": blocks}
+
+
+_FIT_COLS = ("c0", "c1", "c2", "s", "u_star", "se", "min", "lo", "hi")
+
+
+def profile_report_text(prof: dict) -> str:
+    """result/profile.txt of Replay.profile's dict, or result/profile_joint.txt of joint.profile_replays' (which has "recs"). A header
+    line of key value pairs (for a joint profile the recordings and candidates; the replays, the jobs, the wall time, the refinement's
+    status, the steps n and each parameter's step); the centre line (its roll,pitch,yaw [deg] and x,y,z [m], its total lag and shift
+    [ms], its MME and, joint, the recordings' MMEs); a column line and one fixed-column row per profile point in evaluation order (the
+    parameter, k, its offset in the parameter's unit, then the as-run valid queries, MME and replay time, per recording for a joint
+    profile after the joint MME); a column line and one fit line per parameter: `fit`, or `joint` and `rec<b>` for a joint profile, the
+    parameter, its verdict and unit, c0 c1 c2, s, u* and se [steps], the minimum and the interval lo hi in the unit, whether the centre
+    lies inside it, and the lowest profile point's k and MME difference to the centre."""
+    from .profiles import H_LAG_MS, H_ROT_DEG, H_TRANS_M, UNITS
+    c = prof["centre"]
+    joint = "recs" in prof
+    B = len(prof["recs"]) if joint else 1
+    head = (f"recordings {B} candidates {len(prof['rows'])} " if joint else "") + (
+        f"replays {len(prof['rows']) * B} jobs {prof['jobs']} wall_s {prof['wall_s']:.6f} status {prof['status']} steps {prof['steps']} "
+        f"h_rot_deg {H_ROT_DEG:.6f} h_trans_m {H_TRANS_M:.6f} h_lag_ms {H_LAG_MS:.6f}")
+    centre = f"centre {_euler_t(c['R'], c['T'])} lag_ms {c['lag_s'] * 1000.0:.6f} shift_ms {c['shift_s'] * 1000.0:.6f} mme {c['mme']:.9f}"
+    if joint:
+        centre += " mmes " + ",".join("%.9f" % m for m in c["mmes"])
+    cols = ["param", "k", "offset"] + (["mme"] + [f"{x}_{b}" for b in range(B) for x in ("valid", "mme", "seconds")] if joint else
+                                       ["valid", "mme", "seconds"])
+    lines = ["profile " + head, centre, "%-7s %3s %16s" % tuple(cols[:3]) + "".join(" %15s" % x for x in cols[3:])]
+    for r in prof["rows"]:
+        line = "%-7s %3d %16.9f" % (r["param"], r["k"], r["offset"])
+        if joint:
+            line += " %15.9f" % r["mme"]
+        results, secs = (r["results"], r["seconds"]) if joint else ([r["result"]], [r["seconds"]])
+        for res, sec in zip(results, secs):
+            line += " %15d %15.9f %15.3f" % (res["valid"], res["mme"], sec)
+        lines.append(line)
+    lines.append("%-6s %-7s %-10s %-4s" % ("who", "param", "verdict", "unit") + "".join(" %16s" % x for x in _FIT_COLS)
+                 + " %13s %7s %16s" % ("centre_inside", "lower_k", "lower_dmme"))
+    whos = [("joint", prof["fits"])] + [(f"rec{b}", f) for b, f in enumerate(prof["recs"])] if joint else [("fit", prof["fits"])]
+    for who, fits in whos:
+        for p, f in fits.items():
+            vals = (*f["c"], f["s"], f["u"], f["se"], f["u_phys"], f["lo_phys"], f["hi_phys"])
+            lines.append("%-6s %-7s %-10s %-4s" % (who, p, f["verdict"], UNITS[p.split("_")[0]]) + "".join(" %16.9e" % v for v in vals)
+                         + " %13d %7d %16.9e" % (int(f["centre_inside"]), f["lower_k"], f["lower_dmme"]))
+    return "\n".join(lines) + "\n"
+
+
+def parse_profile_report(text: str) -> dict:
+    """The inverse of profile_report_text: {"header": {...}, "centre": {"euler_deg", "t_m" (tuples), "lag_ms", "shift_ms", "mme" and,
+    joint, "mmes"}, "rows": [{"param", "k", "offset", "valid", "mme", "seconds"}, or for a joint profile {"param", "k", "offset", "mme",
+    "valid", "mmes", "seconds" (lists per recording)}] in evaluation order, "fits": {param: {"verdict", "unit", "c0", ..., "hi",
+    "centre_inside", "lower_k", "lower_dmme"}} or, joint, {"joint" or b: {param: ...}}}, or {"nothing": True}."""
+    if text == NOTHING:
+        return {"nothing": True}
+    ls = text.splitlines()
+    h = ls[0].split()
+    assert h[0] == "profile", ls[0]
+    header = {h[i]: (h[i + 1] if h[i] == "status" else float(h[i + 1]) if "." in h[i + 1] else int(h[i + 1])) for i in range(1, len(h), 2)}
+    joint = "recordings" in header
+    B = header["recordings"] if joint else 1
+    f = ls[1].split()
+    assert f[0] == "centre", ls[1]
+    e, t = (tuple(float(x) for x in v.split(",")) for v in f[1:3])
+    centre = dict(euler_deg=e, t_m=t, **{f[i]: float(f[i + 1]) for i in range(3, 9, 2)})
+    if joint:
+        centre["mmes"] = [float(x) for x in f[10].split(",")]
+    n = header["candidates"] if joint else header["replays"]
+    rows = []
+    for line in ls[3:3 + n]:
+        f = line.split()
+        row = dict(param=f[0], k=int(f[1]), offset=float(f[2]))
+        if joint:
+            row.update(mme=float(f[3]), valid=[int(x) for x in f[4::3]], mmes=[float(x) for x in f[5::3]],
+                       seconds=[float(x) for x in f[6::3]])
+        else:
+            row.update(valid=int(f[3]), mme=float(f[4]), seconds=float(f[5]))
+        rows.append(row)
+    fits = {}
+    for line in ls[4 + n:]:
+        f = line.split()
+        fit = dict(verdict=f[2], unit=f[3], **{k: float(x) for k, x in zip(_FIT_COLS, f[4:13])})
+        fit.update(centre_inside=bool(int(f[13])), lower_k=int(f[14]), lower_dmme=float(f[15]))
+        who = "fit" if f[0] == "fit" else "joint" if f[0] == "joint" else int(f[0][3:])
+        fits.setdefault(who, {})[f[1]] = fit
+    return {"header": header, "centre": centre, "rows": rows, "fits": fits["fit"] if not joint else fits}

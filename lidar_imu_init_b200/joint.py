@@ -2,7 +2,7 @@
 
     python -m lidar_imu_init_b200.joint --config CFG --bag A --bag B [...] --out DIR [--devices 0,1,...] [--replay-jobs K]
                                         [--max-candidates N] [--param NAME=VALUE ...] [--max-map-points N] [--assess-radius R]
-                                        [--assess-max-points N] [--assess-replay-max-points N] [--quiet]
+                                        [--assess-max-points N] [--assess-replay-max-points N] [--profile] [--quiet]
 
 Whether an axis of the extrinsic is observable depends on the motion of a recording; several recordings with different excitation
 constrain what one leaves flat. Each recording b is played as `run --config CFG --bag <b> --out DIR/rec<b>` plays it, writing the same
@@ -18,6 +18,9 @@ expanded into its replays, and all of them run at once over every recording's co
 its --replay-jobs - 1 workers live on device devices[b % len(devices)] (--devices, default 0). Writes DIR/result/refinement_joint.txt
 (assess.joint_report_text). Exits 1 with a message on a config, bag or library error, a recording that does not reach the hand-over or
 whose replay store is truncated, the same bag given twice, or a bad --devices, --replay-jobs or --max-candidates.
+
+--profile then replays a profile through the refined calibration along each of its seven parameters, on every recording, and fits
+where each profile has its minimum, for the joint score and for each recording (profile_replays): DIR/result/profile_joint.txt.
 """
 from __future__ import annotations
 
@@ -120,6 +123,34 @@ def refine_replays(replays, finals, max_candidates=None, jobs: int = 1) -> dict:
     return out
 
 
+def profile_replays(replays, ref, jobs: int = 1, steps=None) -> dict:
+    """profiles.profile around refine_replays' result `ref` over the joint score: every candidate (R, T, s) replayed frozen by recording
+    b at the shift s + offsets[b], all of them at once (assess.run_across); the centre's joint and per-recording MMEs are ref's. Returns
+    profile's dict for the joint mean with, on every row, "mmes", "results" and "seconds" (per recording, in recording order); and "recs"
+    (per recording, profiles.fit_all of its own MMEs: which recording pins which parameter, at no extra replay), "wall_s", "jobs",
+    "replays" (all recordings') and "status" (the refinement's)."""
+    from . import profiles as pf
+    B = len(replays)
+    kept = []
+
+    def score_many(cands):
+        runs = assess.run_across([(replays[b], (R, T, s + ref["offsets"][b], True)) for R, T, s in cands for b in range(B)], jobs)
+        kept[:] = [runs[i * B:(i + 1) * B] for i in range(len(cands))]
+        return [_mean([r["result"]["mme"] for r in rs]) for rs in kept]
+    n = pf.STEPS if steps is None else steps
+    t0 = time.perf_counter()
+    out = pf.profile(score_many, ref["R"], ref["T"], ref["shift_s"], ref["mme"], n, lag0=ref["lag0"])
+    out["wall_s"] = time.perf_counter() - t0
+    for row, rs in zip(out["rows"], kept):
+        row["mmes"] = [float(r["result"]["mme"]) for r in rs]
+        row["results"], row["seconds"] = [r["result"] for r in rs], [r["seconds"] for r in rs]
+    c = out["centre"]
+    c["mmes"] = [float(m) for m in ref["mmes"]]
+    out["recs"] = [pf.fit_all([row["mmes"][b] for row in out["rows"]], c["mmes"][b], c["T"], c["lag_s"], n) for b in range(B)]
+    out.update(jobs=jobs, replays=len(out["rows"]) * B, status=ref["status"])
+    return out
+
+
 # ---- the command line ------------------------------------------------------------------------------------------------------------------
 def parse_args(argv=None):
     ap = argparse.ArgumentParser(prog="python -m lidar_imu_init_b200.joint", description=__doc__.split("\n\n")[0],
@@ -140,6 +171,8 @@ def parse_args(argv=None):
                     help=f"LIO points each recording's assessment store keeps (default {assess.MAX_POINTS})")
     ap.add_argument("--assess-replay-max-points", type=int, default=assess.REPLAY_MAX_POINTS, metavar="N",
                     help=f"raw LIO-phase points each recording's replay store keeps (default {assess.REPLAY_MAX_POINTS})")
+    ap.add_argument("--profile", action="store_true", help="after the refinement, replay a profile through the result along each "
+                    "parameter and fit where its minimum lies, jointly and per recording: DIR/result/profile_joint.txt")
     ap.add_argument("--quiet", action="store_true", help="no progress on stderr")
     return ap.parse_args(argv)
 
@@ -230,6 +263,12 @@ def main(argv=None, on_node=None) -> int:
         with open(path, "w") as f:
             f.write(assess.joint_report_text(recs, ref, args.assess_radius, nodes[0].assess.min_neighbors))
         log.info(summary(path, ref, len(nodes), jobs))
+        if args.profile:
+            prof = profile_replays([nd.replay for nd in nodes], ref, jobs)
+            path = os.path.join(args.out, "result", "profile_joint.txt")
+            with open(path, "w") as f:
+                f.write(assess.profile_report_text(prof))
+            log.info(run.profile_summary(path, prof, jobs))
         return 0
     except run.errors() + (JointError,) as e:
         sys.stderr.write(f"error: {e}\n")

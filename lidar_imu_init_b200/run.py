@@ -5,7 +5,7 @@
                                       [--record-compression none|bz2] [--record-topics a,b,...]] [--debug-logs]
                                       [--assess] [--assess-cloud PATH [--assess-cloud-leaf L]] [--assess-radius R]
                                       [--assess-max-points N] [--assess-time] [--assess-replay] [--assess-replay-max-points N]
-                                      [--refine [--refine-max-replays N]]
+                                      [--refine [--refine-max-replays N] [--profile]]
 
 --bag is a ROS1 bag (v2.0), a rosbag2 directory (sqlite3 storage) or one of its .db3 files, told apart by the file's first bytes. The
 LiDAR topic carries livox_ros_driver/CustomMsg or livox_ros_driver2/CustomMsg (lidar_type 1) or sensor_msgs/PointCloud2 in a ROS1
@@ -34,6 +34,9 @@ DIR/result/assessment_replay.txt (stores the LIO scans like --assess).
 sharpest, starting from the better of LI-Init's result and the final extrinsic, within --refine-max-replays replays (default 120). It
 writes every replay, the end condition of each axis and the refined calibration, in the format of Initialization_result.txt, to
 DIR/result/refinement.txt, and leaves Initialization_result.txt as it is.
+--profile (with --refine) then replays a profile through the refined calibration along each of its seven parameters (rotation about
+each IMU axis, translation along it, the lag), 6 steps each side, and fits where each profile has its minimum: a verdict and an
+interval per parameter in degrees, metres and milliseconds, written to DIR/result/profile.txt (profiles.py).
 """
 from __future__ import annotations
 
@@ -45,6 +48,7 @@ import time
 from . import assess as assessmod
 from . import bagwrite
 from . import config as cfgmod
+from . import profiles as profilesmod
 from . import refine as refinemod
 from . import rosbag, rosbag2, rosmsg
 
@@ -91,6 +95,8 @@ def parse_args(argv=None):
     ap.add_argument("--refine", action="store_true", help="search, by LIO replay, for the lag and extrinsic whose map is sharpest and "
                     "write the refined calibration: DIR/result/refinement.txt (records the replay like --assess-replay)")
     ap.add_argument("--refine-max-replays", metavar="N", help=f"replays the refinement may spend (default {refinemod.MAX_REPLAYS})")
+    ap.add_argument("--profile", action="store_true", help="after --refine, replay a profile through the refined calibration along "
+                    "each parameter and fit where its minimum lies: DIR/result/profile.txt")
     ap.add_argument("--replay-jobs", metavar="K", help="replays of --assess-replay and --refine run at once, each on its own device "
                     "context sharing the recorded replay (default 1)")
     return ap.parse_args(argv)
@@ -202,6 +208,8 @@ def main(argv=None, on_node=None) -> int:
     log = Log(quiet=args.quiet)
     try:
         max_replays = refine_max_replays(args) if args.refine else None
+        if args.profile and not args.refine:
+            raise cfgmod.ConfigError("--profile profiles the refined calibration: it needs --refine")
         jobs = replay_jobs(args)
         replaying = args.assess_replay or args.refine
         node, wall = play(args, log, on_node, jobs)      # (closed: the error paths below have nothing left to close)
@@ -238,6 +246,13 @@ def main(argv=None, on_node=None) -> int:
                 log.warn(f"{path}: {assessmod.NOTHING.strip()}")
             else:
                 log.info(refine_summary(path, ref, jobs))
+            if args.profile:
+                path = os.path.join(args.out, "result", "profile.txt")
+                prof = node.replay.write_profile(path, ref)
+                if prof is None:
+                    log.warn(f"{path}: {assessmod.NOTHING.strip()}")
+                else:
+                    log.info(profile_summary(path, prof, jobs))
         if replaying:
             node.replay.close()
         node.odom.g.close()
@@ -264,6 +279,20 @@ def refine_summary(path: str, ref: dict, jobs: int = 1) -> str:
             f"job{'s' if jobs > 1 else ''}); lag "
             f"{ref['lag0'] * 1000.0:.3f} -> {ref['time_lag'] * 1000.0:.3f} ms; from {ref['start']}: rotation {np.degrees(np.arccos(c)):.4f} deg, "
             f"translation {np.linalg.norm(ref['T'] - s['T']) * 1000.0:.2f} mm; MME {s['mme']:.6f} -> {ref['mme']:.6f}")
+
+
+def profile_summary(path: str, prof: dict, jobs: int = 1) -> str:
+    """The profile's summary line: the replays and jobs, then per parameter its verdict and the interval of its minimum in its unit;
+    a `pinned` fit whose minimum lies a step or more from the profile's lowest point (profiles.off_lowest) says so."""
+    parts = []
+    for p, f in prof["fits"].items():
+        unit = profilesmod.UNITS[p.split("_")[0]]
+        iv = f" [{f['lo_phys']:.4f}, {f['hi_phys']:.4f}] {unit}" if f["verdict"] in ("pinned", "edge") else ""
+        if f["verdict"] == "pinned" and profilesmod.off_lowest(f):
+            iv += f" (off the profile's lowest point, k {f['lower_k']:+d}: the parabola misfits)"
+        parts.append(f"{p} {f['verdict']}{iv}")
+    return (f"profile written to {path}: {prof['replays']} replays in {prof['wall_s']:.1f} s ({jobs} replay job{'s' if jobs > 1 else ''}); "
+            + ", ".join(parts))
 
 
 def _abort(node, writer):
